@@ -1,5 +1,5 @@
 #!/usr/bin/env python
-"""bench.py — headline benchmark of the B200-native XIVO inner loop.
+"""bench.py — headline benchmark of the CUDA-native XIVO inner loop.
 
 Metric (BASELINE.json): VIO frames/s on synthetic 640x480 + 200 Hz IMU streams, whole job.
 Workload (BASELINE.json configs[1]): full VIO, 640x480 pinhole, 150 tracked features, EKF state
@@ -12,7 +12,9 @@ one frame (+ its 8 IMU samples) for every sequence on every GPU.
 
 Prints ONE JSON line (rank 0).  `value` = frames/s with the frames already resident in HBM;
 `e2e` = the same through the estimator-level C ABI with pinned HOST frames (H2D inside the timed
-region, pose read back every step).  `roofline` describes the kernel with the largest share of
+region, pose read back every step).  `--dump-outputs DIR` writes what the device-resident pass computed in its last
+step (poses, motion states, counters and a seeded sample of covariances of every sequence) as DIR/<name>.npy; the inputs are
+seeded, so two builds run with the same arguments can be compared output for output.  `roofline` describes the kernel with the largest share of
 device time (CUDA-event durations recorded by the library on its launch streams) in a third pass over
 the next frames of the same streams, in which the batches are stepped one after another so that an
 event pair measures the kernel and not the queueing behind other batches' kernels.
@@ -40,7 +42,7 @@ WORKLOAD = "BASELINE configs[1]: full VIO 640x480 pinhole + 200 Hz IMU, 150 trac
 METRIC = "VIO frames/sec (640x480 synthetic + 200 Hz IMU)"
 # --config: the other full-pipeline workloads BASELINE.json names (parity cases of tests/test_gpu_estimator.py); the driver's runs use 1
 CONFIGS = {
-    1: dict(cfg="vio_640x480.json", G=4, F=14, seqs=1024, streams=32, workload=WORKLOAD, metric=METRIC),  # 1024 x 32: profiles/r02w_sweep.txt
+    1: dict(cfg="vio_640x480.json", G=4, F=14, seqs=1024, streams=32, workload=WORKLOAD, metric=METRIC),
     2: dict(cfg="tumvi_512_equidistant.json", G=15, F=30, seqs=256, streams=8,
             workload="BASELINE configs[2]: TUM-VI equidistant 512x512 + 200 Hz IMU, 200 tracked features, state dim 203 (G=15,F=30)",
             metric="VIO frames/sec (512x512 equidistant synthetic + 200 Hz IMU)"),
@@ -95,8 +97,8 @@ def measured_peaks():
     p = os.path.join(ROOT, "MEASURED_PEAKS.json")
     if os.path.exists(p):
         d = json.load(open(p))
-        return dict(hbm=d.get("hbm_gbs", 6650.0), tf=d.get("bf16_tflops_sustained", 1400.0), src="MEASURED_PEAKS.json (sustained)")
-    return dict(hbm=6650.0, tf=1590.0, src="fallback B200_PROFILING.md")
+        return dict(hbm=d.get("hbm_gbs", 3350.0), tf=d.get("bf16_tflops_sustained", 989.0), src="MEASURED_PEAKS.json (sustained)")
+    return dict(hbm=3350.0, tf=989.0, src="H100 SXM data sheet: HBM3 3.35 TB/s, dense BF16 989 TFLOP/s (700 W card)")
 
 
 class ClockSampler:
@@ -330,7 +332,7 @@ def build_roofline(prof, K, peaks, seqs_per_launch, pass_ms):
     if upd_ms:
         merged["ekf_update"] = dict(calls=kern.get("ekf_gain", {}).get("calls", 0), ms=upd_ms, work=kern.get("ekf_update", {}).get("work", 0))
     if not merged:
-        return dict(kernel=None, bound=None, achieved=None, peak=None, unit=None, frac=None, traffic=None, kernels={}), host_phases
+        return dict(kernel=None, bound=None, achieved=None, peak=None, unit=None, frac=None, kernels={}), host_phases
     tot_ms = sum(v["ms"] for v in merged.values()) or 1.0
     dom = max(merged, key=lambda k: merged[k]["ms"])
     d = merged[dom]
@@ -341,15 +343,6 @@ def build_roofline(prof, K, peaks, seqs_per_launch, pass_ms):
         achieved, peak, unit = work_per_launch / per_launch_s / 1e9, peaks["hbm"], "GB/s"
     else:
         achieved, peak, unit = work_per_launch / per_launch_s / 1e12, peaks["tf"], "TFLOP/s"
-    traffic, traffic_src = None, None
-    try:  # ncu-measured DRAM bytes per launch of that kernel (profiles/), scaled to this run's sequences per launch
-        tname = "r02_traffic.json"
-        tj = json.load(open(os.path.join(ROOT, "profiles", tname)))
-        if dom in tj:
-            traffic = tj[dom] * (seqs_per_launch / tj["sequences_per_launch"])
-            traffic_src = "ncu dram__bytes_{read,write}.sum at %d sequences/launch (profiles/%s), scaled to %d" % (tj["sequences_per_launch"], tname, seqs_per_launch)
-    except Exception:
-        pass
     per_kernel = {}
     for k_, v_ in merged.items():  # the same arithmetic for every kernel with algorithmic work attributed (SURVEY.md §8d, csrc/estimator.cu add_work sites)
         if not v_.get("work") or not v_["ms"]:
@@ -365,13 +358,39 @@ def build_roofline(prof, K, peaks, seqs_per_launch, pass_ms):
     if upd and upd["calls"]:
         ekf_update = dict(us_per_frame=round(upd["ms"] * 1e3 / (upd["calls"] * seqs_per_launch), 4), us_per_launch=round(upd["ms"] * 1e3 / upd["calls"], 3),
                           filters_per_launch=seqs_per_launch, launches=upd["calls"], kernels="ekf_gain_kernel + ekf_cov_kernel (or ekf_cov_tc_kernel)")
-    roofline = dict(kernel=dom, bound=bound, achieved=achieved, peak=peak, unit=unit, frac=achieved / peak, traffic=traffic, traffic_source=traffic_src, peak_source=peaks["src"],
+    roofline = dict(kernel=dom, bound=bound, achieved=achieved, peak=peak, unit=unit, frac=achieved / peak, peak_source=peaks["src"],
                     per_kernel=per_kernel, ekf_update=ekf_update,
                     share_of_device_time=d["ms"] / tot_ms, launches=d["calls"], avg_launch_us=per_launch_s * 1e6,
                     kernels={k: dict(ms=round(v["ms"], 4), calls=v["calls"], share=round(v["ms"] / tot_ms, 4)) for k, v in merged.items()},
                     device_busy_frac=tot_ms / pass_ms, profiled_pass_ms_per_step=pass_ms / K,
                     attribution="third pass, batches stepped one after another (event durations = kernels, not queueing behind other batches)")
     return roofline, host_phases
+
+
+DUMP_P_SAMPLE = 64        # covariances written by --dump-outputs: a seeded sample of this many sequences (all of them up to this count)
+DUMP_LIMIT_BYTES = 64 << 20
+
+
+def dump_outputs(out_dir, bts, sizes):
+    """What a caller of the timed path (xivo_batch_step + the read-back accessors) receives after the last step, for every sequence of
+    this rank in batch order: pose gsb, motion state (V, bg, ba, Rsg), the counters, and the full covariance P of a fixed seeded sample of
+    sequences (p_sample_seq = their indices).  float64 throughout; the total stays under DUMP_LIMIT_BYTES."""
+    os.makedirs(out_dir, exist_ok=True)
+    seqs = [(b_, s) for b_, n in zip(bts, sizes) for s in range(n)]
+    out = dict(gsb=np.stack([b_.gsb(s) for b_, s in seqs]))
+    motion = [b_.motion(s) for b_, s in seqs]
+    for k, name in enumerate(("velocity", "bias_gyro", "bias_accel", "Rsg")):
+        out[name] = np.stack([m[k] for m in motion])
+    out["counters"] = np.array([list(b_.counters(s).values()) for b_, s in seqs], dtype=np.float64)
+    pick = np.sort(np.random.default_rng(0).choice(len(seqs), min(DUMP_P_SAMPLE, len(seqs)), replace=False))
+    out["p_sample_seq"] = pick.astype(np.float64)
+    out["p_sample"] = np.stack([seqs[i][0].P(seqs[i][1]) for i in pick])
+    total = sum(v.nbytes for v in out.values())
+    if total > DUMP_LIMIT_BYTES:
+        raise SystemExit(f"--dump-outputs: {total} bytes exceed the {DUMP_LIMIT_BYTES}-byte limit")
+    for name, v in out.items():
+        np.save(os.path.join(out_dir, name + ".npy"), np.ascontiguousarray(v, dtype=np.float64))
+    log("outputs of the last timed step written to", out_dir, {k: v.shape for k, v in out.items()})
 
 
 def run_ours(args):
@@ -381,8 +400,7 @@ def run_ours(args):
     budget_all = cpu_budget()
     budget = max(1, budget_all // lws)
     # one driver per batch needs a CPU of its own: with a small budget (e.g. a node quota shared by 8 ranks) run fewer batches
-    # a batch needs a driver thread; at least a quarter of the CPUs stay with the workers.  (Half, the rule until r02ae, turned the 12 CPUs a
-    # rank gets on a multi-GPU box into 6 batches of 171 sequences: two waves of the CTA-per-filter kernels on 148 SMs.)
+    # a batch needs a driver thread; at least a quarter of the CPUs stay with the workers
     args.batches = max(1, min(args.batches, budget * 3 // 4))
     os.environ.setdefault("XIVO_THREADS", str(max(1, min(args.max_threads, budget) - args.batches + 1 - args.cpu_headroom)))
     os.environ.setdefault("XIVO_DRIVERS", str(args.batches))
@@ -394,7 +412,7 @@ def run_ours(args):
     if world != args.gpus and world > 1:
         raise SystemExit(f"--gpus {args.gpus} but WORLD_SIZE={world}")
     cfg = load_cfg()
-    cfg["covariance_update"] = args.cov_update  # "fp64" (default, exact parity) or "tf32x3" (tcgen05 downdate, fp32 accuracy)
+    cfg["covariance_update"] = args.cov_update  # "fp64" (default, exact parity) or "tf32x3" (wgmma tensor-core downdate, fp32 accuracy)
     B, K, W, FPS, CH = args.seqs, args.steps, args.warmup, args.frames_per_step, args.channels
     S0 = max(1, min(args.streams, B))
     # ---- synthetic inputs (rendered before CUDA is initialised: fork pool) ----
@@ -549,6 +567,8 @@ def run_ours(args):
     # profiler off (its event records and locks cost ~1 ms/step); the third only attributes time to kernels
     r_dev = timed(True, 0, K)
     log("device-resident pass", r_dev["ms"], "ms")
+    if args.dump_outputs and rank == 0:
+        dump_outputs(args.dump_outputs, bts, sizes)
     L.xivo_set_frame_ingest.restype = C.c_int
 
     def cal_step(k):
@@ -671,13 +691,14 @@ def main():
     ap.add_argument("--channels", type=int, default=1, choices=[1, 3], help="1 = grey frames (default), 3 = BGR like the reference's cv::imread input (src/app/vio.cpp:72)")
     ap.add_argument("--profile-steps", type=int, default=4, help="steps of the (serial, slow) kernel-attribution pass")
     ap.add_argument("--profile-overlapped", action="store_true", help="attribution pass with the batches in flight together (event durations then include queueing)")
-    ap.add_argument("--max-threads", type=int, default=16, help="cap on host threads per rank (workers + drivers): more than this measured slower (SCALE_r01: 88 threads 2.3x slower than 16)")
+    ap.add_argument("--max-threads", type=int, default=16, help="cap on host threads per rank (workers + drivers)")
     ap.add_argument("--no-single-stream", dest="single_stream", action="store_false", help="skip the batch-of-one latency measurement")
     ap.add_argument("--cpu-cores", type=int, default=0)
-    ap.add_argument("--cov-update", default="fp64", choices=["fp64", "tf32x3"], help="arithmetic of the covariance downdate (tf32x3 = tcgen05 tensor cores)")
+    ap.add_argument("--cov-update", default="fp64", choices=["fp64", "tf32x3"], help="arithmetic of the covariance downdate (tf32x3 = 3xTF32 on the tensor cores)")
     ap.add_argument("--no-cpu-baseline", action="store_true")
     ap.add_argument("--no-numa", dest="numa", action="store_false", help="leave the process on every allowed CPU instead of the NUMA node of its GPU")
-    ap.add_argument("--prefetch", action="store_true", help="e2e pass with xivo_batch_prefetch_frames (the upload of frame k + 1 is started before frame k is processed); measured neutral on the B200 box (profiles/r02z_sweep.txt), so the default is the plain call")
+    ap.add_argument("--prefetch", action="store_true", help="e2e pass with xivo_batch_prefetch_frames (the upload of frame k + 1 is started before frame k is processed)")
+    ap.add_argument("--dump-outputs", metavar="DIR", default=None, help="write what the timed device-resident pass computed in its last step as DIR/<name>.npy")
     ap.add_argument("--ingest", default="auto", choices=["auto"] + list(INGEST_MODES), help="how pinned host frames reach the device (e2e pass); auto = calibrate both before the timed region")
     args = ap.parse_args()
     if args.warmup < 3:

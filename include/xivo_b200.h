@@ -1,5 +1,5 @@
 /*
- * xivo_b200.h — C ABI of the B200-native XIVO inner loop.
+ * xivo_b200.h — C ABI of the CUDA-native (H100, sm_90a) XIVO inner loop.
  *
  * The reference (ucla-vision/xivo) has no FFI/plugin layer: its boundary is the C++ class API
  * (src/estimator.h:115-231, src/tracker.h:25-54) and the pybind11 module
@@ -113,7 +113,7 @@ int xivo_ekf_update(xivo_ctx* ctx, int N, int M, const double* H, double* P, con
                     double* err);
 
 /* Same update with options.  XIVO_UPDATE_TF32X3: the rank-M covariance downdate P -= K (H P) runs on the
- * tensor cores (tcgen05.mma kind::tf32, operands split hi+lo = "3xTF32", fp32 accumulator in TMEM) instead of
+ * tensor cores (wgmma.mma_async .tf32, operands split hi+lo = "3xTF32", fp32 accumulator in registers) instead of
  * fp64 CUDA cores: the "fp32 covariance" mode (BASELINE configs[2]); gain, innovation and the storage of P stay
  * fp64.  Tolerance vs the fp64 update: |dP| <= 1e-5 * max|P| (tests/test_gpu_ekf.py). */
 #define XIVO_UPDATE_TF32X3 1u

@@ -1,5 +1,5 @@
 """EKF measurement update at the BASELINE state sizes, B filters per launch, through xivo_ekf_update_batch and the in-library CUDA-event
-profiler: ms per launch of the gain kernel and of the covariance downdate (fp64 CUDA cores / tcgen05 3xTF32), Joseph-equivalent and
+profiler: ms per launch of the gain kernel and of the covariance downdate (fp64 CUDA cores / wgmma 3xTF32), Joseph-equivalent and
 executed flop rates, and the fp64 traffic of P that bounds the downdate.  usage: python scripts/kbench_update.py [B]"""
 import ctypes as C, json, os, sys
 import numpy as np
@@ -10,7 +10,7 @@ L = capi.lib()
 ctx = capi.Context(0)
 B = int(sys.argv[1]) if len(sys.argv) > 1 else 512
 peaks = json.load(open(os.path.join(os.path.dirname(os.path.dirname(os.path.abspath(__file__))), "MEASURED_PEAKS.json"))) if os.path.exists("MEASURED_PEAKS.json") else {}
-hbm, tf = peaks.get("hbm_gbs", 6574.1), peaks.get("bf16_tflops_sustained", 1404.6)
+hbm, tf = peaks.get("hbm_gbs", 3350.0), peaks.get("bf16_tflops_sustained", 989.0)  # fallback: H100 SXM data sheet
 
 def report():
     buf = C.create_string_buffer(1 << 16)
@@ -26,7 +26,7 @@ for N, M in ((89, 28), (203, 60), (299, 124)):
     H = rng.normal(size=(B, M, N)) * (rng.uniform(size=(B, M, N)) < 0.09)
     inn = rng.normal(size=(B, M))
     R = np.ones((B, M))
-    for mode, env in (("fp64", {}), ("tf32x3 (tcgen05, TMA-staged operands)", {}), ("tf32x3 first kernel", {"XIVO_TC_V1": "1"})):
+    for mode, env in (("fp64", {}), ("tf32x3 (wgmma, TMA-staged operands)", {}), ("tf32x3 first kernel", {"XIVO_TC_V1": "1"})):
         os.environ.pop("XIVO_TC_V1", None)
         os.environ.update(env)
         tc = mode != "fp64"

@@ -43,7 +43,6 @@ def test_roofline_picks_dominant_kernel_and_computes_achieved():
     pk = r["per_kernel"]
     assert set(pk) == {"lk_track", "pyrdown", "imu_cov_propagate", "ekf_update"}
     assert pk["ekf_update"]["bound"] == "tensor" and abs(pk["ekf_update"]["achieved"] - 100 * 64 * 4.4e6 / 8e-3 / 1e12) < 1e-3
-    assert r["traffic"] is None or r["traffic"] > 0  # profiles/r01_traffic.json scaled to 64 sequences per launch
     json.dumps(r)  # serialisable
 
 

@@ -70,7 +70,7 @@ def test_dense_update_matches_joseph(ctx, N, M):
 
 @pytest.mark.parametrize("N,M", [(89, 24), (203, 60), (299, 124), (23, 2), (130, 33)])
 def test_dense_update_tensor_core_tf32x3(ctx, N, M):
-    """XIVO_UPDATE_TF32X3: the downdate P -= K (HP) on tcgen05 tensor cores (3xTF32, fp32 accumulate in TMEM).
+    """XIVO_UPDATE_TF32X3: the downdate P -= K (HP) on wgmma tensor cores (3xTF32, fp32 accumulate in registers).
     Tolerance (stated in include/xivo_b200.h): fp32-level, |dP_ij| <= 1e-5 sqrt(P_ii P_jj) elementwise and
     1e-5 max|P|; gain / err are the fp64 kernels, hence identical."""
     rng = np.random.default_rng(N + M)
@@ -97,7 +97,7 @@ def test_dense_update_tensor_core_tf32x3(ctx, N, M):
 def test_batched_update_both_tensor_core_kernels_and_fp64(ctx, N, M, B, monkeypatch):
     """xivo_ekf_update_batch: B filters in one launch pair.  fp64 path against the Joseph oracle per filter; the tensor-core downdate in
     both formulations -- ekf_cov_tc2_kernel (default: TF32 hi / lo operands written by the gain kernel, TMA-staged, several column chunks
-    per CTA, double-buffered TMEM accumulators) and the first kernel (XIVO_TC_V1=1) -- at the stated fp32 tolerance, exactly symmetric,
+    per CTA, MMAs of the next chunk overlapping the epilogue) and the first kernel (XIVO_TC_V1=1) -- at the stated fp32 tolerance, exactly symmetric,
     and equal to each other to fp32 rounding.  Sizes: the three BASELINE state dimensions with their maximal measurement counts, a
     measurement count that is not a multiple of the 32-row K block, and a state dimension that crosses one 128-row tile by 2 rows."""
     rng = np.random.default_rng(N * 7 + M + B)

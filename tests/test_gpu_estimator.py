@@ -103,7 +103,7 @@ def test_pcw_trajectory_matches_the_reference_estimator(case, tmp_path):
 
 
 def test_pcw_trajectory_tensor_core_covariance():
-    """"covariance_update": "tf32x3" — the downdate of every measurement update runs on tcgen05 tensor cores with
+    """"covariance_update": "tf32x3" — the downdate of every measurement update runs on wgmma tensor cores with
     fp32-level accuracy (BASELINE configs[2] "fp32 covariance").  Stated tolerance against the fp64 oracle after
     3 s (75 updates): position 1e-4 m, rotation 1e-5, covariance 1e-4 * max|P|; the in-state id tables stay exact."""
     G, F = 15, 30

@@ -1,6 +1,6 @@
-"""xivo_b200 — B200-native implementation of XIVO's per-frame visual-inertial inner loop.
+"""xivo_b200 — CUDA-native implementation of XIVO's per-frame visual-inertial inner loop.
 
-The product is libxivo_b200.so (hand-written sm_100a CUDA behind the C ABI of
+The product is libxivo_b200.so (hand-written sm_90a CUDA behind the C ABI of
 include/xivo_b200.h).  This package only binds it (ctypes) and mirrors the reference's
 pyxivo surface; it contains no CPU implementation of the hot path.
 """

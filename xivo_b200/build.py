@@ -1,4 +1,4 @@
-"""Builds libxivo_b200.so in-tree with nvcc for sm_100a (no torch dependency in the library)."""
+"""Builds libxivo_b200.so in-tree with nvcc for sm_90a (no torch dependency in the library)."""
 from __future__ import annotations
 
 import os
@@ -9,7 +9,7 @@ HERE = os.path.dirname(os.path.abspath(__file__))
 CSRC = os.path.join(HERE, "csrc")
 LIB = os.path.join(HERE, "libxivo_b200.so")
 NVCC = os.environ.get("NVCC", "/usr/local/cuda/bin/nvcc")
-ARCH = ["-gencode", "arch=compute_100a,code=sm_100a"]
+ARCH = ["-gencode", "arch=compute_90a,code=sm_90a"]
 COMMON = ["-O3", "-std=c++17", "-lineinfo", "-Xcompiler", "-fPIC,-pthread", "-Xptxas", "-v"]
 
 # (source, extra flags).  The tracker is compiled without FMA contraction so its float math

@@ -759,8 +759,8 @@ __global__ void __launch_bounds__(IMU_THREADS) imu_cov_propagate_kernel(int N, d
 // Second formulation of the same algebra (identical operation order per element): every thread owns fixed elements — a strip
 // thread keeps its FK[q] / A[q] of all stages of the sub-step in registers, a P thread keeps its covariance entries in registers —
 // so the Runge-Kutta combinations need no shared-memory round trip and no index tables, and the stage chain has two barriers per
-// stage (double-buffered Acc / SA / CV) instead of three.  ncu of the first formulation: 29 % of stall samples at barriers,
-// IMAD/LDS/ISETP index traffic 39 % of the issued instructions, DFMA 6 % (profiles/r01c_source_summaries.txt).
+// stage (double-buffered Acc / SA / CV) instead of three.  (A formulation with shared-memory index tables spends its issue slots on
+// index arithmetic and its stalls at barriers rather than on DFMA.)
 __device__ __forceinline__ double v_block(const F9s& f, const ImuConst& c, int e) {  // (R diag(qa) R^T)[e / 3][e % 3]
   const int i = e / 3, j = e - 3 * i;
   return f.R[3 * i] * c.qimu[3] * f.R[3 * j] + f.R[3 * i + 1] * c.qimu[4] * f.R[3 * j + 1] + f.R[3 * i + 2] * c.qimu[5] * f.R[3 * j + 2];

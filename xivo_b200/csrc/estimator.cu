@@ -45,7 +45,7 @@ extern std::atomic<unsigned long long> g_launches;
 // How pinned host frames reach the frame ring: 0 = one gather launch whose SMs read the host memory over PCIe,
 // 1 = one cudaMemcpyAsync per frame on the copy engine.  Results are identical; which is faster depends on the
 // host's PCIe path, so it is a run-time setting (xivo_set_frame_ingest; initial value from XIVO_ZEROCOPY).
-// Default: the copy engine (with the tables of every phase fetched by kernels, DMA frames delay them least: profiles/r02i_burst_probe.txt).
+// Default: the copy engine (with the tables of every phase fetched by kernels, DMA frames delay them least).
 static std::atomic<int> g_frame_ingest{(getenv("XIVO_ZEROCOPY") && getenv("XIVO_ZEROCOPY")[0] == '1') ? 0 : 1};
 
 // Pinned host mirror + device array.
@@ -110,8 +110,7 @@ struct Mirror {
 // Completion of a stream without CUDA calls in the wait loop: the driver thread asks the stream to write a ticket number into mapped
 // pinned memory behind everything enqueued so far (cuStreamWriteValue32, fetched from the driver at run time; a one-thread kernel where
 // the driver lacks it) and then polls that word.  Why: every runtime call of a driver thread contends with the calls of the other
-// batches' drivers -- measured on the B200 box (profiles/r02g_api_probe.txt), the runtime sustains ~0.7 M calls/s in total however many
-// threads issue them, and threads spinning on cudaEventQuery slow the issuing threads down by a further third.
+// batches' drivers (the runtime serialises them), and threads spinning on cudaEventQuery slow the issuing threads down further.
 typedef CUresult (*StreamWriteValue32Fn)(CUstream, CUdeviceptr, cuuint32_t, unsigned int);
 static StreamWriteValue32Fn stream_write_value32() {
   static StreamWriteValue32Fn fn = [] {
@@ -126,8 +125,7 @@ static StreamWriteValue32Fn stream_write_value32() {
 }
 // Upload of a host-written table blob by the SMs: 16-byte loads from the mapped pinned copy, stores to the device copy.  Why not the
 // copy engine: the frames of a step travel by DMA, and a small cudaMemcpyAsync issued behind that burst waits for it in the engine's
-// FIFO -- measured on the B200 box (profiles/r02i_burst_probe.txt): 750 us for a 165 KB table round trip behind the 157 MB frame burst
-// of one step against 112 us when a kernel reads the table in place (31 / 27 us on an idle link).
+// FIFO, while a kernel that reads the table in place does not queue behind the burst.
 // Four loads in flight per thread: the reads cross PCIe (2-3 us each on an idle link, far more while a frame burst holds it), so the
 // number of round trips, not the byte count, is what a table upload costs.
 __global__ void __launch_bounds__(256) fetch_kernel(const uint4* __restrict__ src, uint4* __restrict__ dst, unsigned n16) {
@@ -687,12 +685,12 @@ class Batch {
     if (gather) {
       XB_CUDA(up_blob(blobG, blobG.n, st_copy));  // [sources | ring offsets]
       // host sources: one warp per frame with four loads in flight still fills the link when several batches pull at once, and hogs it
-      // less for the other batches' table fetches than wider grids do (profiles/r02i_burst_probe.txt)
+      // less for the other batches' table fetches than wider grids do
       if (int rc = launch_gather_frames(st_copy, ingest_ptr.d, dRing, 0, ingest_off.d, ib, B, on_device ? 64 : 1, on_device ? 256 : 32)) return rc;
       g_launches += 1;
     } else {
       // copy engine: runs of sequences whose sources are evenly spaced (frames of one pinned pool) and whose ring slots agree go down as
-      // ONE pitched copy each (measured on the B200 box: 55 GB/s for pitched copies of 307 KB rows against 32 GB/s for one call per frame)
+      // ONE pitched copy each (far fewer copy calls than one per frame)
       int s = 0;
       while (s < B) {
         int e = s + 1;
@@ -1852,7 +1850,7 @@ static int choose_lanes(const Json& cfg, int n_seq) {
     const char* e = getenv("XIVO_LANES");
     L = e && *e ? atoi(e) : 0;
   }
-  if (L <= 0) L = 1;  // measured (profiles/r02e_sweep.txt): several lock-step batch handles on the shared worker pool beat lanes (103 k vs 75 k frames/s), so lanes are opt-in
+  if (L <= 0) L = 1;  // several lock-step batch handles on the shared worker pool beat lanes, so lanes are opt-in
   return std::max(1, std::min(L, n_seq));
 }
 

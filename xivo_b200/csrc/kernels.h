@@ -103,12 +103,12 @@ int launch_ekf_update(cudaStream_t st, EkfLayout lay, const FeatJac* jac, const 
 int launch_ekf_update_dense(cudaStream_t st, int N, int M, const double* H, const double* diagR, const double* inn, double* P,
                             double* err, double* HP, double* Kt, int batch, int tensor_core = 0, const TcOperands* tc = nullptr);
 
-// Tensor-core (tcgen05, 3xTF32, fp32 accumulator in TMEM) form of the downdate P -= Kt^T HP (ekf_tc_kernels.cu);
+// Tensor-core (wgmma, 3xTF32, fp32 accumulator in registers) form of the downdate P -= Kt^T HP (ekf_tc_kernels.cu);
 // selected by tensor_core != 0 in the two launchers above.  ekf_cov_tc_fault: 1 if a kernel ever gave up waiting
 // for its MMAs (never expected), -1 on a CUDA error.
 int launch_ekf_cov_tc(cudaStream_t st, int N, const int* nsel, int Mdense, int Mmax, const double* HP, const double* Kt, double* P,
                       int batch);
-// Second formulation (ekf_cov_tc2_kernel): the gain kernel also writes K^T and HP as TF32 hi/lo words in the UMMA canonical layout
+// Second formulation (ekf_cov_tc2_kernel): the gain kernel also writes K^T and HP as TF32 hi/lo words in the wgmma canonical K-major layout
 // [filter][hi|lo][k/4][state column (Npad)][4]; the downdate kernel stages them by TMA.
 struct TcOperands {
   uint32_t* kt32 = nullptr;

@@ -4,7 +4,7 @@
 // float math in LK is compiled with -fmad=false so it rounds like the scalar CPU code.
 //
 // All kernels take a batch dimension (blockIdx.z or .y = independent sequence) because the
-// only way a 640x480 frame fills a B200 is by processing many sequences per launch.
+// only way a 640x480 frame fills an H100 (132 SMs) is by processing many sequences per launch.
 #include <cuda.h>
 #include <algorithm>
 #include <cstdlib>
@@ -51,7 +51,7 @@ int launch_gather_frames(cudaStream_t st, const uint8_t* const* src, uint8_t* ds
                          size_t bytes, int batch, int max_chunks, int threads) {
   ProfScope ps("gather_frames", st);
   // max_chunks: CTAs per frame.  Host sources (pinned memory read over PCIe): a few small CTAs with four loads in flight per thread already
-  // saturate the link (50.7 GB/s from 8 down to 1 CTA per frame, profiles/r02f_pcie_probe.txt) and leave the SMs' thread slots to the
+  // saturate the link and leave the SMs' thread slots to the
   // kernels of the other batches while they wait.
   threads = threads < 32 ? 32 : (threads > 256 ? 256 : (threads & ~31));
   const int chunks = (int)std::min<size_t>(max_chunks < 1 ? 1 : max_chunks, (bytes + (size_t)threads * 16 - 1) / ((size_t)threads * 16));
@@ -207,9 +207,8 @@ __global__ void __launch_bounds__(PV_THREADS) pyrdown_vec_kernel(uint8_t* __rest
 // assembly disappear (ncu, round 2 start: 82 % issue-active at 7 % of DRAM peak).  BORDER_REFLECT_101 only concerns the CTAs on the
 // image rim, which patch their halo rows / columns inside shared memory after the box has landed.  The arithmetic that follows is
 // pyrdown_vec_kernel's (byte-permute + dp4a on the same words), so the output is bit-identical.
-// Box geometry (probed on the B200, profiles/r02f_tma_probe.txt): the innermost start coordinate times the element size must be a
-// multiple of 16 bytes -- a box starting at column 2 ox - 4 raises "illegal instruction" -- while negative (aligned) coordinates and
-// boxes that stick out of the tensor are fine.  So the box starts at column 2 ox - 16 and is 160 bytes wide.
+// Box geometry: the innermost start coordinate times the element size is kept a multiple of 16 bytes, while negative (aligned)
+// coordinates and boxes that stick out of the tensor are fine.  So the box starts at column 2 ox - 16 and is 160 bytes wide.
 constexpr int PT_LEAD = 16;                  // source column of tile byte 0 = 2 ox - PT_LEAD
 constexpr int PT_BOXW = 2 * PV_TX + 32;      // 160 bytes: source columns [2 ox - 16, 2 ox + 144)
 constexpr int PT_WORDS = PT_BOXW / 4;        // 40 words per staged row
@@ -385,10 +384,9 @@ constexpr int FT_SW = FT_TX + 2, FT_SH = FT_TY + 2;  // score region
 
 __device__ __forceinline__ int fast_score(const uint8_t (*t)[FT_RW + 4], int rx, int ry, int thr) {
   // t indexed [row][col] in region coords; (rx, ry) is the centre.  Works on the raw ring values
-  // p[k] (no signed differences): nvcc 12.9 / sm_100a was observed on B200 to fuse
-  // max(best, max(mn, -mx)) into a 3-input VIMNMX and drop the negation (the kernel returned
-  // max_k(v - p_k) - 1; see profiles/r01_notes.md), so the only arithmetic here is min/max of plain
-  // operands plus two final subtractions.
+  // p[k] (no signed differences): nvcc 12.9 has been seen to fuse max(best, max(mn, -mx)) into a
+  // 3-input VIMNMX and drop the negation (the kernel returned max_k(v - p_k) - 1), so the only
+  // arithmetic here is min/max of plain operands plus two final subtractions.
   const int v = t[ry][rx];
   const int lo = v - thr, hi = v + thr;
   int p[16];
@@ -652,7 +650,7 @@ __global__ void __launch_bounds__(FT_THREADS) fast_pair_kernel(const uint8_t* __
 // is zero-filled by the TMA unit, which is exactly the value the thread-staged kernel stores there (FAST never scores a pixel closer
 // than 3 to the border, so the fill value is never compared).  The bytes are then widened to the 16-bit tile the packed scoring works
 // on; everything after that is fast_pair_tile, so the keypoints are identical.
-constexpr int FTM_BOXW = 96, FTM_LEAD = 16;  // tile byte 0 = image column ox - 16 (16-byte aligned start: profiles/r02f_tma_probe.txt)
+constexpr int FTM_BOXW = 96, FTM_LEAD = 16;  // tile byte 0 = image column ox - 16 (16-byte aligned start)
 __global__ void __launch_bounds__(FT_THREADS) fast_pair_tma_kernel(const __grid_constant__ CUtensorMap img_map, unsigned long long img_stride,
                                                                    const unsigned long long* __restrict__ seq_off, int rows, int cols, int thr,
                                                                    int nonmax, unsigned* __restrict__ kp_out, int max_kp, int* __restrict__ kp_count,
@@ -1000,8 +998,7 @@ __global__ void __launch_bounds__(LK_WARPS * 32) lk_kernel(const uint8_t* __rest
 // keeps its <= 8 template samples (I, Ix, Iy) in registers for the whole level.  Per iteration a lane
 // loads 2 bytes per sample slot (rows y, y+1 of its column) and gets the x+1 neighbours by shuffle,
 // instead of 4 loads + 3 shared-memory reads; no integer divisions remain in the loops.
-// (6 CTAs of 4 warps per SM at 80 registers.  A 64-register cap for 8 CTAs spills a few words and measured 7 % slower on the B200:
-// 334 against 312 us per launch of 128 sequences, profiles/r02aa_lk_occupancy.txt.)
+// (6 CTAs of 4 warps per SM at 80 registers; a 64-register cap for 8 CTAs spills a few words.)
 template <int WIN, bool PACK>
 __global__ void __launch_bounds__(LK_WARPS * 32, PACK ? 6 : 1) lk_kernel_fast(const uint8_t* __restrict__ prev_pyr, const uint8_t* __restrict__ next_pyr,
                                                                unsigned long long pyr_stride,

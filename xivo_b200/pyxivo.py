@@ -2,7 +2,7 @@
 
 `Estimator` mirrors the method names of the reference's pybind11 module
 (/root/reference/pybind11/pyxivo.cpp:332-398) for the hot path; `Batch` is the lock-step
-multi-sequence form that the B200 needs to be kept busy.  ctypes plumbing only — all computation
+multi-sequence form that the GPU needs to be kept busy.  ctypes plumbing only — all computation
 happens in libxivo_b200.so.
 """
 from __future__ import annotations
