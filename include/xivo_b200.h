@@ -173,7 +173,10 @@ int xivo_cov_propagate(xivo_ctx* ctx, int N, double* P, const double* Phi, const
  * caller integrates; for every Runge-Kutta stage it passes what the motion Jacobian
  * (ComputeMotionJacobianAt, src/estimator.cpp:614-702) depends on:
  *   stage16 : nstages x {Rsb(9), Cg*gyro-bg (3), Ca*accel-ba (3), h}; h = sub-step length on the first
- *             stage of each sub-step, negative when that sub-step closes a Propagate call
+ *             stage of each sub-step, negative when that sub-step closes a Propagate call.  The records
+ *             must come from one such integration: the device rebuilds the Rsb of the later stages of a
+ *             sub-step from its first stage (as the integrator composes them), and their rates from the
+ *             first stage's and the slope between stage 0 and stage 5 (Prince-Dormand) / 1 (RK4)
  *   qimu12 / qmodel23 : diagonals of Qimu (gyro, accel, gyro bias, accel bias) and Qmodel
  *   stages_per_step : 7 (Prince-Dormand) or 4 (RK4) */
 int xivo_imu_cov_propagate(xivo_ctx* ctx, int N, double* P, int nstages, const double* stage16, const double* g3,

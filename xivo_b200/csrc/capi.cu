@@ -522,20 +522,39 @@ int xivo_imu_cov_propagate(xivo_ctx* ctx, int N, double* P, int nstages, const d
              "imu_cov_propagate: bad arguments");
   if (nstages == 0) return XIVO_OK;
   static_assert(sizeof(ImuStage) == 16 * sizeof(double), "ImuStage layout");
+  // The kernel reads one record per sub-step and rebuilds the rotation and rates of its other stages: the sub-step takes R, the rates
+  // and h of its first stage, and the rate slopes from the stage whose rates lie furthest from them (cin = 1 for Prince-Dormand, 1/2 for RK4).
+  const bool pd = stages_per_step == 7;
+  const int nsteps = nstages / stages_per_step, sfar = pd ? 5 : 1;
+  double cs_far, cin_far;
+  imu_stage_coef(pd, sfar, &cs_far, &cin_far);
+  std::vector<ImuStep> steps(nsteps);
+  for (int k = 0; k < nsteps; ++k) {
+    const double* s0 = stage16 + (size_t)16 * stages_per_step * k;
+    const double* sf = s0 + 16 * sfar;
+    ImuStep& r = steps[k];
+    memcpy(r.R, s0, 72); memcpy(r.gc, s0 + 9, 24); memcpy(r.ac, s0 + 12, 24);
+    r.h = s0[15];
+    const double t = cin_far * fabs(r.h);
+    for (int e = 0; e < 3; ++e) {
+      r.dgc[e] = t > 0 ? (sf[9 + e] - s0[9 + e]) / t : 0.0;
+      r.dac[e] = t > 0 ? (sf[12 + e] - s0[12 + e]) / t : 0.0;
+    }
+  }
   cudaStream_t st = ctx->stream;
   ImuConst ic;
   memcpy(ic.g, g3, 24); memcpy(ic.qimu, qimu12, 96); memcpy(ic.qmodel, qmodel23, 184);
   ic.stages_per_step = stages_per_step; ic.pad = 0;
   const int zero = 0;
   DevBuf<double> dP((size_t)N * N);
-  DevBuf<ImuStage> dS(nstages);
+  DevBuf<ImuStep> dS(nsteps);
   DevBuf<ImuConst> dC(1);
   DevBuf<int> dn(1), df(1);
   XB_REQUIRE(dP.ok() && dS.ok() && dC.ok() && dn.ok() && df.ok(), "cudaMalloc failed");
   XB_CUDA(cudaMemcpyAsync(dP.p, P, sizeof(double) * N * N, cudaMemcpyHostToDevice, st));
-  XB_CUDA(cudaMemcpyAsync(dS.p, stage16, sizeof(ImuStage) * nstages, cudaMemcpyHostToDevice, st));
+  XB_CUDA(cudaMemcpyAsync(dS.p, steps.data(), sizeof(ImuStep) * nsteps, cudaMemcpyHostToDevice, st));
   XB_CUDA(cudaMemcpyAsync(dC.p, &ic, sizeof(ic), cudaMemcpyHostToDevice, st));
-  XB_CUDA(cudaMemcpyAsync(dn.p, &nstages, sizeof(int), cudaMemcpyHostToDevice, st));
+  XB_CUDA(cudaMemcpyAsync(dn.p, &nsteps, sizeof(int), cudaMemcpyHostToDevice, st));
   XB_CUDA(cudaMemcpyAsync(df.p, &zero, sizeof(int), cudaMemcpyHostToDevice, st));
   int rc = launch_imu_cov_propagate(st, N, dP.p, dS.p, df.p, dn.p, dC.p, 1);
   if (rc) return rc;

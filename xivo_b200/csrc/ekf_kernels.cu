@@ -550,13 +550,13 @@ int launch_pack_state(cudaStream_t st, int N, const double* P, const double* err
 // ------------------------------------------------------------------------------------------
 // IMU covariance propagation: the covariance side of Estimator::Propagate -> PrinceDormand / RK4
 // (/root/reference/src/estimator.cpp:539-704, src/princedormand.cpp:85-221, src/rk4.cpp:35-103).
-// One warp per filter consumes the per-stage records the host wrote while integrating the nominal
-// state (kernels.h: ImuStage).  Structure used: only the Wsb/Tsb/Vsb rows of F are non-zero, so
-// F*X is a 9 x 23 strip and  Pdot = [A;0] + [A;0]^T + G Q G^T,  A = F[0:9,:] P,  G Q G^T block diagonal
+// One block per filter consumes the per-sub-step records the host wrote while integrating the nominal
+// state (kernels.h: ImuStep) and rebuilds what every Runge-Kutta stage needs from them.  Structure
+// used: only the Wsb/Tsb/Vsb rows of F are non-zero, so F*X is a 9 x 23 strip and  Pdot = [A;0] + [A;0]^T + G Q G^T,  A = F[0:9,:] P,  G Q G^T block diagonal
 // (Q diagonal).  At the end the motion/structure strips get Phi = prod(I + FK h) (rows >= 9 = identity).
 // ------------------------------------------------------------------------------------------
-struct F9s {  // shared-memory image of the non-zero blocks of F and of R
-  double dW[9], dVW[9], dVba[9], dVg[6], R[9];
+struct F9s {  // shared-memory image of the non-zero blocks of F and of R (+ the stage's calibrated rates)
+  double dW[9], dVW[9], dVba[9], dVg[6], R[9], gc[3], ac[3];
 };
 // element (i, j), i < 9, of F[0:9,:] * B for a 23-column B; lt9: rows >= 9 of B are zero
 __device__ __forceinline__ double f9_elem(const F9s& f, const double* B, int i, int j, bool lt9) {
@@ -601,23 +601,59 @@ __constant__ double kBrk[4] = {1.0 / 6, 2.0 / 6, 2.0 / 6, 1.0 / 6};
 
 constexpr int IMU_THREADS = 256;
 constexpr int IMU_CHUNK = 56;
-__global__ void __launch_bounds__(IMU_THREADS) imu_cov_propagate_kernel(int N, double* __restrict__ P, const ImuStage* __restrict__ stages,
-                                                                        const int* __restrict__ first, const int* __restrict__ nstages,
+// Stage images of the n stages [c0, c0 + n) of a filter (c0, n: whole sub-steps of nst stages) from its sub-step records.
+// Pass 1, one thread per stage: the stage's rotation and rates (imu_stage_from_step).  Pass 2, nine threads per stage: the
+// non-zero blocks of F,  dW = -hat(gc), dVW = -R hat(ac), dVba = -R, dVg = (-R hat(g))[:, :2].  sH[q] = the h of stage q's sub-step.
+__device__ __forceinline__ void imu_load_chunk(const ImuStep* __restrict__ stp, int c0, int n, int nst, const ImuConst& c, F9s* sFc, double* sH,
+                                               int tid) {
+  const bool pd = nst == 7;
+  for (int u = tid; u < n; u += IMU_THREADS) {
+    const int k = (c0 + u) / nst, s = (c0 + u) - nst * k;
+    F9s& f = sFc[u];
+    M3 R;
+    V3 gc, ac;
+    imu_stage_from_step(stp[k], s, pd, &R, &gc, &ac);
+#pragma unroll
+    for (int e = 0; e < 9; ++e) f.R[e] = R.m[e];
+#pragma unroll
+    for (int e = 0; e < 3; ++e) { f.gc[e] = gc.v[e]; f.ac[e] = ac.v[e]; }
+    sH[u] = stp[k].h;
+  }
+  __syncthreads();
+  for (int u = tid; u < n * 9; u += IMU_THREADS) {
+    const int q = u / 9, e = u - 9 * q;
+    const int i = e / 3, j = e - 3 * i;
+    F9s& f = sFc[q];
+    const double* Rm = f.R;
+    f.dVba[e] = -Rm[e];
+    f.dW[e] = -hat_elem(f.gc, i, j);
+    double v = 0, vg = 0;
+    for (int k = 0; k < 3; ++k) {
+      v += Rm[3 * i + k] * hat_elem(f.ac, k, j);
+      vg += Rm[3 * i + k] * hat_elem(c.g, k, j);
+    }
+    f.dVW[e] = -v;
+    if (j < 2) f.dVg[2 * i + j] = -vg;
+  }
+}
+
+__global__ void __launch_bounds__(IMU_THREADS) imu_cov_propagate_kernel(int N, double* __restrict__ P, const ImuStep* __restrict__ steps,
+                                                                        const int* __restrict__ first, const int* __restrict__ nsteps,
                                                                         const ImuConst* __restrict__ cst) {
   const int b = blockIdx.x, tid = threadIdx.x;
-  const int nall = nstages[b];
-  if (nall == 0) return;
+  if (nsteps[b] == 0) return;
   __shared__ double sP[529], sP0[529], sA[7][207], sFK[7][207], sSA[207], sAcc[207], sT9[207], sPhi[207], sV[7][9], sCV[9], sGc[23];
   __shared__ ImuConst c;
   __shared__ unsigned char sI[529], sJ[529];  // row / column of a flat 23x23 index (no div/mod in the loops)
   if (tid < (int)(sizeof(ImuConst) / 8)) reinterpret_cast<double*>(&c)[tid] = reinterpret_cast<const double*>(cst + b)[tid];
   for (int t = tid; t < 529; t += IMU_THREADS) { sI[t] = (unsigned char)(t / 23); sJ[t] = (unsigned char)(t % 23); }
   double* __restrict__ Pb = P + (size_t)b * N * N;
-  const ImuStage* __restrict__ stg = stages + first[b];
+  const ImuStep* __restrict__ stp = steps + first[b];
   for (int t = tid; t < 529; t += IMU_THREADS) sP[t] = Pb[(size_t)(t / 23) * N + t % 23];
   for (int t = tid; t < 207; t += IMU_THREADS) sPhi[t] = (t / 23 == t % 23) ? 1.0 : 0.0;
   __syncthreads();
   const int nst = c.stages_per_step;
+  const int nall = nsteps[b] * nst;  // stages
   const bool pd = nst == 7;
   if (tid < 23) {  // state-independent diagonal of G Q G^T
     double v = 0.0;
@@ -627,35 +663,15 @@ __global__ void __launch_bounds__(IMU_THREADS) imu_cov_propagate_kernel(int N, d
     sGc[tid] = v;
   }
   __syncthreads();
-  // Stage records are consumed in chunks of IMU_CHUNK (a multiple of both 7 and 4 stages per substep): the non-zero
-  // blocks of F of every stage of the chunk are built in parallel up front, so the serial stage chain below never
-  // waits on global memory.  dW = -hat(gc), dVW = -R hat(ac), dVba = -R, dVg = (-R hat(g))[:, :2]
+  // Stages are consumed in chunks of IMU_CHUNK (a multiple of both 7 and 4 stages per substep): the non-zero
+  // blocks of F of every stage of the chunk are built in parallel up front (imu_load_chunk), so the serial stage chain below
+  // never waits on global memory or on the stage rotations.
   extern __shared__ __align__(16) unsigned char imu_dyn[];
   F9s* sFc = reinterpret_cast<F9s*>(imu_dyn);
   double* sH = reinterpret_cast<double*>(sFc + IMU_CHUNK);
   auto load_chunk = [&](int c0) {
     __syncthreads();  // the previous chunk is no longer read
-    const int n = min(IMU_CHUNK, nall - c0);
-    for (int u = tid; u < n * 9; u += IMU_THREADS) {
-      const int q = u / 9, e = u - 9 * q;
-      const int i = e / 3, j = e - 3 * i;
-      const double* src = reinterpret_cast<const double*>(stg + c0 + q);
-      const double* Rm = src;
-      const double* gc = src + 9;
-      const double* ac = src + 12;
-      F9s& f = sFc[q];
-      f.R[e] = Rm[e];
-      f.dVba[e] = -Rm[e];
-      f.dW[e] = -hat_elem(gc, i, j);
-      double v = 0, vg = 0;
-      for (int k = 0; k < 3; ++k) {
-        v += Rm[3 * i + k] * hat_elem(ac, k, j);
-        vg += Rm[3 * i + k] * hat_elem(c.g, k, j);
-      }
-      f.dVW[e] = -v;
-      if (j < 2) f.dVg[2 * i + j] = -vg;
-    }
-    for (int u = tid; u < n; u += IMU_THREADS) sH[u] = reinterpret_cast<const double*>(stg + c0 + u)[15];
+    imu_load_chunk(stp, c0, min(IMU_CHUNK, nall - c0), nst, c, sFc, sH, tid);
     __syncthreads();
   };
   const F9s* pf = sFc;
@@ -766,17 +782,16 @@ __device__ __forceinline__ double v_block(const F9s& f, const ImuConst& c, int e
   return f.R[3 * i] * c.qimu[3] * f.R[3 * j] + f.R[3 * i + 1] * c.qimu[4] * f.R[3 * j + 1] + f.R[3 * i + 2] * c.qimu[5] * f.R[3 * j + 2];
 }
 
-__global__ void __launch_bounds__(IMU_THREADS) imu_cov_propagate_v2_kernel(int N, double* __restrict__ P, const ImuStage* __restrict__ stages,
-                                                                           const int* __restrict__ first, const int* __restrict__ nstages,
+__global__ void __launch_bounds__(IMU_THREADS) imu_cov_propagate_v2_kernel(int N, double* __restrict__ P, const ImuStep* __restrict__ steps,
+                                                                           const int* __restrict__ first, const int* __restrict__ nsteps,
                                                                            const ImuConst* __restrict__ cst) {
   const int b = blockIdx.x, tid = threadIdx.x;
-  const int nall = nstages[b];
-  if (nall == 0) return;
+  if (nsteps[b] == 0) return;
   __shared__ double sP[529], sP0[529], sAcc[2][207], sSA[2][207], sPhi[2][207], sCV[2][9], sGc[23];
   __shared__ ImuConst c;
   if (tid < (int)(sizeof(ImuConst) / 8)) reinterpret_cast<double*>(&c)[tid] = reinterpret_cast<const double*>(cst + b)[tid];
   double* __restrict__ Pb = P + (size_t)b * N * N;
-  const ImuStage* __restrict__ stg = stages + first[b];
+  const ImuStep* __restrict__ stp = steps + first[b];
   // ---- fixed ownership
   const bool strip = tid < 207;               // element (si, sj) of the 9 x 23 strips
   const int si = strip ? tid / 23 : 0, sj = strip ? tid - 23 * si : 0;
@@ -797,6 +812,7 @@ __global__ void __launch_bounds__(IMU_THREADS) imu_cov_propagate_v2_kernel(int N
   if (strip) sPhi[0][tid] = si == sj ? 1.0 : 0.0;
   __syncthreads();
   const int nst = c.stages_per_step;
+  const int nall = nsteps[b] * nst;  // stages
   const bool pd = nst == 7;
   if (tid < 23) {  // state-independent diagonal of G Q G^T
     double v = 0.0;
@@ -808,29 +824,9 @@ __global__ void __launch_bounds__(IMU_THREADS) imu_cov_propagate_v2_kernel(int N
   extern __shared__ __align__(16) unsigned char imu_dyn[];
   F9s* sFc = reinterpret_cast<F9s*>(imu_dyn);
   double* sH = reinterpret_cast<double*>(sFc + IMU_CHUNK);
-  auto load_chunk = [&](int c0) {  // as in the first formulation: non-zero blocks of F for IMU_CHUNK stages, built in parallel
+  auto load_chunk = [&](int c0) {  // as in the first formulation
     __syncthreads();
-    const int n = min(IMU_CHUNK, nall - c0);
-    for (int u = tid; u < n * 9; u += IMU_THREADS) {
-      const int q = u / 9, e = u - 9 * q;
-      const int i = e / 3, j = e - 3 * i;
-      const double* src = reinterpret_cast<const double*>(stg + c0 + q);
-      const double* Rm = src;
-      const double* gc = src + 9;
-      const double* ac = src + 12;
-      F9s& f = sFc[q];
-      f.R[e] = Rm[e];
-      f.dVba[e] = -Rm[e];
-      f.dW[e] = -hat_elem(gc, i, j);
-      double v = 0, vg = 0;
-      for (int k = 0; k < 3; ++k) {
-        v += Rm[3 * i + k] * hat_elem(ac, k, j);
-        vg += Rm[3 * i + k] * hat_elem(c.g, k, j);
-      }
-      f.dVW[e] = -v;
-      if (j < 2) f.dVg[2 * i + j] = -vg;
-    }
-    for (int u = tid; u < n; u += IMU_THREADS) sH[u] = reinterpret_cast<const double*>(stg + c0 + u)[15];
+    imu_load_chunk(stp, c0, min(IMU_CHUNK, nall - c0), nst, c, sFc, sH, tid);
     __syncthreads();
   };
   // increment of covariance entry (i, j): strip_sym(SA) + sw * diag(GQG const) + CV on the velocity block
@@ -952,7 +948,7 @@ __global__ void __launch_bounds__(IMU_THREADS) imu_cov_propagate_v2_kernel(int N
 }
 
 // XIVO_IMU_V1=1 routes the propagation through the first formulation (parity tests compare the two)
-int launch_imu_cov_propagate(cudaStream_t st, int N, double* P, const ImuStage* stages, const int* first, const int* nstages,
+int launch_imu_cov_propagate(cudaStream_t st, int N, double* P, const ImuStep* steps, const int* first, const int* nsteps,
                              const ImuConst* cst, int batch) {
   ProfScope ps("imu_cov_propagate", st);
   const size_t dyn = IMU_CHUNK * (sizeof(F9s) + sizeof(double));
@@ -963,8 +959,8 @@ int launch_imu_cov_propagate(cudaStream_t st, int N, double* P, const ImuStage* 
     attr_set = true;
   }
   const char* e = getenv("XIVO_IMU_V1");
-  if (e && e[0] == '1') imu_cov_propagate_kernel<<<batch, IMU_THREADS, dyn, st>>>(N, P, stages, first, nstages, cst);
-  else imu_cov_propagate_v2_kernel<<<batch, IMU_THREADS, dyn, st>>>(N, P, stages, first, nstages, cst);
+  if (e && e[0] == '1') imu_cov_propagate_kernel<<<batch, IMU_THREADS, dyn, st>>>(N, P, steps, first, nsteps, cst);
+  else imu_cov_propagate_v2_kernel<<<batch, IMU_THREADS, dyn, st>>>(N, P, steps, first, nsteps, cst);
   XB_CUDA(cudaGetLastError());
   return 0;
 }

@@ -265,7 +265,7 @@ class Batch {
   Mirror<int> nopsJ, firstJ, nopsU, firstU;
   Mirror<SubfilterIn> sub_in;
   Mirror<SubfilterOut> sub_out;
-  Mirror<ImuStage> stg[2];  // packed stage records of all filters, two staging halves used alternately
+  Mirror<ImuStep> stg[2];  // packed Runge-Kutta sub-step records of all filters, two staging halves used alternately
   Mirror<int> stg_first[2], stg_n[2];
   int stg_half = 0;
   unsigned stg_busy[2] = {0, 0};  // st2 ticket after which the half may be refilled (0 = free)
@@ -334,7 +334,10 @@ class Batch {
     cudaStreamCreateWithFlags(&st2, cudaStreamNonBlocking);
     cudaStreamCreateWithFlags(&st_copy, cudaStreamNonBlocking);
     cudaEventCreateWithFlags(&wait_ev, cudaEventDisableTiming | (lane_mode ? cudaEventBlockingSync : 0));
-    for (int b = 0; b < B; ++b) est.emplace_back(new Estimator(cfg, lay, tracker_only));
+    for (int b = 0; b < B; ++b) {
+      est.emplace_back(new Estimator(cfg, lay, tracker_only));
+      est.back()->compact_records = true;  // imu_cov_propagate rebuilds the intermediate Runge-Kutta stages itself
+    }
     cov_tc = est[0]->c.cov_update_tf32x3 ? 1 : 0;
     use_1pt = est[0]->c.use_1pt_RANSAC;
     table_order.resize(B);
@@ -389,15 +392,15 @@ class Batch {
           opsU.adopt(H(o4), D(o4), nB * maxops);
         }
       }
-      for (int h = 0; h < 2 && ok; ++h) {  // IMU stage records: [first | n | stages ...], two staging halves
+      for (int h = 0; h < 2 && ok; ++h) {  // IMU sub-step records: [first | n | steps ...], two staging halves
         Carve c;
         const size_t o0 = c.take(nB * 4), o1 = c.take(nB * 4);
         blobI_fixed = c.off;
-        const size_t o2 = c.take(nB * kMaxStages * sizeof(ImuStage));
+        const size_t o2 = c.take(nB * kMaxSteps * sizeof(ImuStep));
         ok = ok && blobI[h].alloc_fetchable((c.off + 15) & ~(size_t)15);
         if (ok) {
           stg_first[h].adopt(blobI[h].h + o0, blobI[h].d + o0, nB); stg_n[h].adopt(blobI[h].h + o1, blobI[h].d + o1, nB);
-          stg[h].adopt(blobI[h].h + o2, blobI[h].d + o2, nB * kMaxStages);
+          stg[h].adopt(blobI[h].h + o2, blobI[h].d + o2, nB * kMaxSteps);
         }
       }
     }
@@ -483,18 +486,18 @@ class Batch {
     *total = n;
     return 0;
   }
-  // Enqueue the covariance algebra of the queued Runge-Kutta stage records of the given sequences
+  // Enqueue the covariance algebra of the queued Runge-Kutta sub-step records of the given sequences
   // (imu_cov_propagate_kernel).  Asynchronous: the host already holds the propagated nominal state.
   int integrate(const std::vector<int>& act) {
     HostScope hsi("issue_integrate");
     cudaStream_t st = st2;
     bool any = false;
-    for (int b : act) any = any || !est[b]->stages.empty();
+    for (int b : act) any = any || !est[b]->steps.empty();
     if (!any) return 0;
     // A queue longer than the per-filter staging capacity (an IMU / vision gap of several hundred ms: the reference integrates any dt,
     // estimator.cpp:539-592) goes down in several launches of whole sub-steps each; the kernel composes per launch.
     const int sps = std::max(1, icst.h[act[0]].stages_per_step);
-    const int chunk = (kMaxStages / sps) * sps;
+    const int chunk = kMaxStages / sps;  // sub-steps per launch
     std::vector<size_t> cur(B, 0);
     for (;;) {
       const int h = stg_half;
@@ -508,23 +511,23 @@ class Batch {
       bool more = false;
       for (int b : act) {
         Estimator& e = *est[b];
-        const int n = (int)std::min<size_t>((size_t)chunk, e.stages.size() - cur[b]);
+        const int n = (int)std::min<size_t>((size_t)chunk, e.steps.size() - cur[b]);
         if (n <= 0) continue;
         stg_first[h].h[b] = total;
         stg_n[h].h[b] = n;
         total += n;
       }
       if (!total) break;
-      // the records themselves (~20 KB per sequence and frame) are copied by the pool, not by the driver thread alone
+      // the records themselves (~5 KB per sequence and frame) are copied by the pool, not by the driver thread alone
       pfor(act, [&](int b, int) {
         const int n = stg_n[h].h[b];
-        if (n > 0) memcpy(stg[h].h + stg_first[h].h[b], est[b]->stages.data() + cur[b], sizeof(ImuStage) * n);
+        if (n > 0) memcpy(stg[h].h + stg_first[h].h[b], est[b]->steps.data() + cur[b], sizeof(ImuStep) * n);
       });
       for (int b : act) {
         cur[b] += stg_n[h].h[b];
-        more = more || cur[b] < est[b]->stages.size();
+        more = more || cur[b] < est[b]->steps.size();
       }
-      XB_CUDA(up_blob(blobI[h], blobI_fixed + (size_t)total * sizeof(ImuStage), st));
+      XB_CUDA(up_blob(blobI[h], blobI_fixed + (size_t)total * sizeof(ImuStep), st));
       if (int rc = launch_imu_cov_propagate(st, N, dP, stg[h].d, stg_first[h].d, stg_n[h].d, icst.d, B)) return rc;
       stg_busy[h] = tk2.next + 1;  // the next ticket of st2 lies behind this launch
       stg_half ^= 1;
@@ -532,13 +535,13 @@ class Batch {
       {
         int nact = 0;
         for (int b = 0; b < B; ++b) nact += stg_n[h].h[b] > 0;
-        // algorithmic bytes: the stage records + the motion block read and written + the 23 x (N-23) strip read, 9 rows of it written (twice: mirrored)
-        Prof::get().add_work("imu_cov_propagate", total * (double)sizeof(ImuStage) + nact * 8.0 * (2 * 529 + (23 + 18) * (double)(N - 23)));
+        // algorithmic bytes: the sub-step records + the motion block read and written + the 23 x (N-23) strip read, 9 rows of it written (twice: mirrored)
+        Prof::get().add_work("imu_cov_propagate", total * (double)sizeof(ImuStep) + nact * 8.0 * (2 * 529 + (23 + 18) * (double)(N - 23)));
       }
       if (!more) break;
     }
     for (int b : act) {
-      est[b]->stages.clear();
+      est[b]->steps.clear();
       est[b]->prop_pending = false;
     }
     return 0;

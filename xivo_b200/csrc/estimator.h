@@ -442,9 +442,15 @@ class Estimator {
   double Pmm[529];  // host mirror of the motion block of P
   double Phi[529];  // pending strip transition (product of per-substep F)
   bool prop_pending = false;
-  std::vector<ImuStage> stages;  // Runge-Kutta stage records whose covariance algebra has not run on the device yet
-  // the queue must be flushed to the device before it can overflow (one Propagate call adds <= ~256 records)
-  bool needs_state_now() const { return (int)stages.size() > kMaxStages - 320; }
+  // Runge-Kutta records whose covariance algebra has not run on the device yet: one per stage (the default), or, with
+  // compact_records (set by Batch, whose kernel rebuilds the intermediate stages), one per sub-step
+  std::vector<ImuStage> stages;
+  std::vector<ImuStep> steps;
+  bool compact_records = false;
+  int stages_per_step = 7;  // 7 = Prince-Dormand, 4 = RK4
+  int pending_stages() const { return (int)stages.size() + (int)steps.size() * stages_per_step; }
+  // the queue must be flushed to the device before it can overflow (one Propagate call adds <= ~256 stages)
+  bool needs_state_now() const { return pending_stages() > kMaxStages - 320; }
   std::vector<EditOp> edits;  // pending covariance edits, in order
   std::vector<double> diagP;  // last downloaded diagonal of P
   std::vector<char> gsel, fsel;
@@ -531,6 +537,7 @@ class Estimator {
   void propagate(bool visual_meas);
   void compose_motion(MotionX& Xs, const V3& V, const V3& gyro, const V3& accel, double dt) const;
   static void compose_motion_core(M3& Rsb, V3& Tsb, V3& Vsb, const V3& V, const V3& gc, const V3& ac, const V3& g_s, double dt);
+  static V3 stage_velocity(const M3& Rsb, const V3& Vsb, const V3& ac, const V3& g_s, double dt);
   void record_stage(const M3& Rsb, const V3& gc, const V3& ac, double h_enc);
   void nominal_step(bool pd, const V3& gyro0, const V3& accel0, double h, bool closes_call);
   void integrate_nominal(const V3& gyro0, const V3& accel0, double dt);

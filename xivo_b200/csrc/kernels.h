@@ -4,6 +4,7 @@
 #pragma once
 #include <cuda.h>
 #include "common.cuh"
+#include "hostmath.h"
 
 namespace xb {
 
@@ -158,22 +159,53 @@ namespace xb {
 // ---------------- IMU covariance propagation on device (ekf_kernels.cu) ----------------
 // The nominal motion state is a short, strictly sequential fp64 chain (sin/cos, quaternion
 // renormalisation) — a CPU core runs it ~30x faster than one GPU thread — so the host integrates it and
-// records, for every Runge-Kutta stage, what the motion Jacobian depends on.  The device does the
-// covariance algebra (23x23 block + strips) of all filters in parallel from those records.
-struct ImuStage {
+// records what the motion Jacobian depends on.  The device does the covariance algebra (23x23 block +
+// strips) of all filters in parallel from those records.
+struct ImuStage {  // one Runge-Kutta stage (public ABI of xivo_imu_cov_propagate; the estimator's full records)
   double R[9];   // Rsb at the stage
   double gc[3];  // calibrated gyro  Cg*gyro - bg
   double ac[3];  // calibrated accel Ca*accel - ba
   double h;      // sub-step length, stored on the FIRST stage of each sub-step; negative = this sub-step closes a
                  // Propagate call (add Qmodel afterwards, src/estimator.cpp:590)
 };
+// One Runge-Kutta sub-step in the form the kernel reads: what the device cannot derive.  Stage s of the sub-step has the rates
+// gc + dgc * (cin_s |h|), ac + dac * (cin_s |h|) and the rotation so3_normalize(R so3_exp(gc_s * cs_s |h|)) (stage 0: R itself),
+// with the cs / cin of Estimator::nominal_step (imu_stage_coef); the kernel rebuilds them in parallel.  22 doubles per sub-step
+// instead of 7 x 16 (Prince-Dormand) or 4 x 16 (RK4).
+struct ImuStep {
+  double R[9];    // Rsb at the start of the sub-step
+  double gc[3];   // calibrated gyro  Cg*gyro - bg at the start of the sub-step
+  double ac[3];   // calibrated accel Ca*accel - ba at the start of the sub-step
+  double dgc[3];  // Cg * slope_gyro
+  double dac[3];  // Ca * slope_accel
+  double h;       // sub-step length; negative = this sub-step closes a Propagate call (as ImuStage::h)
+};
+// (cs, cin) of stage s >= 1: the stage composes the rotation over cs*h with the rates at cin*h (Prince-Dormand: cin = cs; RK4 of
+// the reference: cin = 1/2 for every stage, rk4.cpp:79)
+__host__ __device__ inline void imu_stage_coef(bool pd, int s, double* cs, double* cin) {
+  *cs = pd ? (s == 1 ? 2.0 / 9 : s == 2 ? 3.0 / 9 : s == 3 ? 5.0 / 9 : s == 4 ? 6.0 / 9 : 1.0) : (s < 3 ? 0.5 : 1.0);
+  *cin = pd ? *cs : 0.5;
+}
+// Rotation and calibrated rates of stage s of a sub-step record, as Estimator::nominal_step composes them when it writes one record
+// per stage (the kernel rebuilds every stage this way)
+__host__ __device__ inline void imu_stage_from_step(const ImuStep& r, int s, bool pd, M3* R, V3* gc, V3* ac) {
+  for (int e = 0; e < 9; ++e) R->m[e] = r.R[e];
+  for (int e = 0; e < 3; ++e) { gc->v[e] = r.gc[e]; ac->v[e] = r.ac[e]; }
+  if (s == 0) return;
+  double cs, cin;
+  imu_stage_coef(pd, s, &cs, &cin);
+  const double h = fabs(r.h);
+  for (int e = 0; e < 3; ++e) { gc->v[e] += r.dgc[e] * (cin * h); ac->v[e] += r.dac[e] * (cin * h); }
+  *R = so3_normalize(m3_mul(*R, so3_exp(v3_scale(*gc, cs * h))));
+}
 constexpr int kMaxStages = 1024;  // per filter between two flushes (one Propagate call with dt = 40 ms needs 140)
+constexpr int kMaxSteps = kMaxStages / 4;  // the same capacity in sub-steps (RK4: 4 stages per sub-step; Prince-Dormand uses 146)
 struct ImuConst {  // per filter
   double g[3], qimu[12], qmodel[23];
   int stages_per_step;  // 7 = Prince-Dormand, 4 = RK4
   int pad;
 };
-// stages: packed; filter b reads stages[first[b] .. first[b] + nstages[b])
-int launch_imu_cov_propagate(cudaStream_t st, int N, double* P, const ImuStage* stages, const int* first /*B*/, const int* nstages /*B*/,
+// steps: packed; filter b reads steps[first[b] .. first[b] + nsteps[b])
+int launch_imu_cov_propagate(cudaStream_t st, int N, double* P, const ImuStep* steps, const int* first /*B*/, const int* nsteps /*B*/,
                              const ImuConst* cst /*B*/, int batch);
 }  // namespace xb
