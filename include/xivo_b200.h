@@ -115,7 +115,10 @@ int xivo_ekf_update(xivo_ctx* ctx, int N, int M, const double* H, double* P, con
 /* Same update with options.  XIVO_UPDATE_TF32X3: the rank-M covariance downdate P -= K (H P) runs on the
  * tensor cores (wgmma.mma_async .tf32, operands split hi+lo = "3xTF32", fp32 accumulator in registers) instead of
  * fp64 CUDA cores: the "fp32 covariance" mode (BASELINE configs[2]); gain, innovation and the storage of P stay
- * fp64.  Tolerance vs the fp64 update: |dP| <= 1e-5 * max|P| (tests/test_gpu_ekf.py). */
+ * fp64.  Tolerance vs the fp64 update, elementwise: |dP_ij| <= 1e-5 * sqrt(P_ii P_jj) (tests/test_gpu_ekf.py, tests/test_gpu_ekf_batch.py).
+ * Measured on an H100 80GB HBM3 (400 W limit) with estimator-like H (feature Jacobians sharing group columns) and variances from 1e-8 to
+ * 1: at most 1.3e-6 for ekf_cov_tc2_kernel and 2.2e-6 for the first kernel (N = 299, M up to 124), consistent with the 3xTF32 product
+ * error 2^-22 sum_k |K_ik||HP_kj| (up to 1.2e-6 of sqrt(P_ii P_jj) on these inputs) plus the fp32 accumulation. */
 #define XIVO_UPDATE_TF32X3 1u
 int xivo_ekf_update_ex(xivo_ctx* ctx, int N, int M, const double* H, double* P, const double* inn, const double* diagR,
                        double* err, unsigned flags);
@@ -134,6 +137,26 @@ int xivo_filter_update(xivo_ctx* ctx, int G, int F, const double* camera, const 
                        int n, const double* feat_x, const double* feat_xp, const int* feat_ref_sind,
                        const int* feat_sind, const int* sel, int nsel, double R, double* P, double* err,
                        double* H_dense);
+
+/* The gate and update phases of the estimator for `batch` filters of one layout (G, F), run `npass` times in a row on the same device
+ * buffers, with the launches and arguments Estimator batches use (Jacobian / gate kernel with the pre-gate edit list, then the gain and
+ * downdate kernels with the post-gate edit list).  The TF32 operand buffers of XIVO_UPDATE_TF32X3 are zeroed once per call, not between
+ * passes, as in a running estimator.
+ *   per filter b     : camera (11), X24 (24), groups (G x 12), nfeat[b] <= F features in feat_x (F x 3), feat_xp (F x 2),
+ *                      feat_ref / feat_sind (F), Rmeas[b], the initial covariance P (N x N)
+ *   per pass p and b : pre_nops[p * batch + b] ops of the pre-gate list, post_nops[...] of the post-gate list, nsel[p * batch + b]
+ *                      indices into the feature table at sel + (p * batch + b) * F.  The ops of both lists are packed in (pass, filter)
+ *                      order, in the xivo_cov_edit format (4 ints + 9 doubles each)
+ *   flags            : XIVO_UPDATE_TF32X3, XIVO_UPDATE_FULL_J (stack the rows of J unchanged, as the 1-point RANSAC update does,
+ *                      instead of Feature::FillJacobianBlock's layout); XIVO_TC_V1=1 in the environment selects the first tensor-core kernel
+ * Outputs after every pass: P_out (npass x batch x N x N), err (npass x batch x N; NaN where S was not positive definite, the filter's P
+ * then keeps its post-gate value), mh (npass x batch x F; 0 beyond nfeat), diag (npass x batch x N: diag(P) after the pre-gate edits). */
+#define XIVO_UPDATE_FULL_J 2u
+int xivo_filter_update_batch(xivo_ctx* ctx, int G, int F, int batch, int npass, const double* camera, const double* X24,
+                             const double* groups, const int* nfeat, const double* feat_x, const double* feat_xp, const int* feat_ref,
+                             const int* feat_sind, const double* Rmeas, const double* P, const int* pre_nops, const int* pre_ops,
+                             const double* pre_blk, const int* nsel, const int* sel, const int* post_nops, const int* post_ops,
+                             const double* post_blk, unsigned flags, double* P_out, double* err, double* mh, double* diag);
 
 /* Depth sub-filter for n not-in-state features; replaces Feature::SubfilterUpdate
  * (src/feature.cpp:246-297).  ref: n x {Rsb(9) Tsb(3)} of each feature's reference group. */

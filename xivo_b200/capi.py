@@ -222,6 +222,50 @@ class Context:
         )
         return P, err, Hd
 
+    def filter_update_batch(self, G, F, filters, passes, tf32x3=False, full_j=False):
+        """The estimator's gate + update phases for B filters of one layout, len(passes) times on the same device buffers.
+        filters: B dicts with camera, X24, groups (G x 12), feat_x (n x 3), feat_xp (n x 2), feat_ref, feat_sind (n), R, P (N x N).
+        passes: per pass, B dicts with "pre" / "post" edit lists of (type, a, b, n[, blk9]) ops and "sel" (indices into the features).
+        Returns P (npass, B, N, N), err (npass, B, N), mh (npass, B, F), diag (npass, B, N) after every pass."""
+        B, npass, N = len(filters), len(passes), 23 + 6 * G + 3 * F
+        cam = np.zeros((B, 11)); X = np.zeros((B, 24)); grp = np.zeros((B, G, 12)); R = np.zeros(B); P0 = np.zeros((B, N, N))
+        fx = np.zeros((B, F, 3)); fxp = np.zeros((B, F, 2)); fr = np.zeros((B, F), np.int32); fs = np.zeros((B, F), np.int32)
+        nfeat = np.zeros(B, np.int32)
+        for b, f in enumerate(filters):
+            n = len(f["feat_x"])
+            cam[b], X[b], grp[b], R[b], P0[b], nfeat[b] = f["camera"], f["X24"], f["groups"], f["R"], f["P"], n
+            fx[b, :n], fxp[b, :n], fr[b, :n], fs[b, :n] = f["feat_x"], f["feat_xp"], f["feat_ref"], f["feat_sind"]
+
+        def pack(key):
+            counts, ops, blks = np.zeros((npass, B), np.int32), [], []
+            for p, ps in enumerate(passes):
+                assert len(ps) == B
+                for b, d in enumerate(ps):
+                    lst = d.get(key, [])
+                    counts[p, b] = len(lst)
+                    for op in lst:
+                        ops.append(op[:4])
+                        blks.append(np.ravel(op[4]) if len(op) > 4 else np.zeros(9))
+            return counts, _i32(np.reshape(ops, (-1, 4))), _f64(np.reshape(blks, (-1, 9)))
+
+        pre_n, pre_ops, pre_blk = pack("pre")
+        post_n, post_ops, post_blk = pack("post")
+        nsel, sel = np.zeros((npass, B), np.int32), np.zeros((npass, B, F), np.int32)
+        for p, ps in enumerate(passes):
+            for b, d in enumerate(ps):
+                s = np.asarray(d.get("sel", []), np.int32)
+                nsel[p, b] = len(s)
+                sel[p, b, : len(s)] = s
+        Po, err, mh, diag = np.zeros((npass, B, N, N)), np.zeros((npass, B, N)), np.zeros((npass, B, F)), np.zeros((npass, B, N))
+        flags = (1 if tf32x3 else 0) | (2 if full_j else 0)
+        _check(
+            lib().xivo_filter_update_batch(self._h, G, F, B, npass, _p(cam), _p(X), _p(grp), _p(nfeat), _p(fx), _p(fxp), _p(fr), _p(fs), _p(R),
+                                           _p(P0), _p(pre_n), _p(pre_ops), _p(pre_blk), _p(nsel), _p(sel), _p(post_n), _p(post_ops), _p(post_blk),
+                                           C.c_uint(flags), _p(Po), _p(err), _p(mh), _p(diag)),
+            "xivo_filter_update_batch",
+        )
+        return Po, err, mh, diag
+
     def subfilter_batch(self, camera, X24, x, P33, xp, ref, outlier, Rtri, mh_thresh):
         camera, X24 = _f64(camera), _f64(X24)
         x, P33, xp, ref, outlier = _f64(x).reshape(-1, 3), _f64(P33).reshape(-1, 9), _f64(xp).reshape(-1, 2), _f64(ref).reshape(-1, 12), _f64(outlier)

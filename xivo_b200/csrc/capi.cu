@@ -389,6 +389,123 @@ int xivo_filter_update(xivo_ctx* ctx, int G, int F, const double* camera, const 
   return XIVO_OK;
 }
 
+// Packs n edit ops (xivo_cov_edit format) into out, checking them against the state dimension.
+static int pack_edits(int N, const int* ops, const double* blk, int n, EditOp* out) {
+  for (int i = 0; i < n; ++i) {
+    EditOp& h = out[i];
+    h.type = ops[4 * i]; h.a = ops[4 * i + 1]; h.b = ops[4 * i + 2]; h.n = ops[4 * i + 3];
+    XB_REQUIRE(h.type >= 0 && h.type <= 2, "filter_update_batch: unknown edit op");
+    const int w = h.type == 2 ? 3 : h.n;
+    XB_REQUIRE(w >= 0 && h.a >= 0 && h.a + w <= N && (h.type != 1 || (h.b >= 0 && h.b + w <= N)), "filter_update_batch: edit op out of range");
+    for (int k = 0; k < 9; ++k) h.blk[k] = (blk && h.type == 2) ? blk[9 * i + k] : 0.0;
+  }
+  return 0;
+}
+
+// The gate + update phases of Batch (estimator.cu: process_visual) for `batch` filters, `npass` times on the same device buffers.
+int xivo_filter_update_batch(xivo_ctx* ctx, int G, int F, int batch, int npass, const double* camera, const double* X24, const double* groups,
+                             const int* nfeat, const double* feat_x, const double* feat_xp, const int* feat_ref, const int* feat_sind,
+                             const double* Rmeas, const double* P, const int* pre_nops, const int* pre_ops, const double* pre_blk,
+                             const int* nsel, const int* sel, const int* post_nops, const int* post_ops, const double* post_blk, unsigned flags,
+                             double* P_out, double* err, double* mh, double* diag) {
+  API_BEGIN;
+  XB_REQUIRE((flags & ~(unsigned)(XIVO_UPDATE_TF32X3 | XIVO_UPDATE_FULL_J)) == 0, "filter_update_batch: unknown flags");
+  XB_REQUIRE(G > 0 && F > 0 && batch > 0 && npass > 0 && camera && X24 && groups && nfeat && feat_x && feat_xp && feat_ref && feat_sind && Rmeas &&
+                 P && pre_nops && nsel && sel && post_nops && P_out && err && mh && diag,
+             "filter_update_batch: bad arguments");
+  const EkfLayout lay{G, F};
+  const int N = lay.N(), Mmax = 2 * F;
+  const size_t nb = (size_t)batch, NN = (size_t)N * N;
+  for (int b = 0; b < batch; ++b) {
+    XB_REQUIRE(nfeat[b] >= 0 && nfeat[b] <= F, "filter_update_batch: need 0 <= nfeat <= F");
+    for (int i = 0; i < nfeat[b]; ++i) {
+      const size_t fi = (size_t)b * F + i;
+      XB_REQUIRE(feat_ref[fi] >= 0 && feat_ref[fi] < G && feat_sind[fi] >= 0 && feat_sind[fi] < F, "filter_update_batch: slot index out of range");
+    }
+  }
+  // edit lists of every pass, packed in (pass, filter) order; first* / n*: npass x batch
+  std::vector<int> first_pre(npass * nb), first_post(npass * nb);
+  int npre = 0, npost = 0;
+  for (size_t q = 0; q < npass * nb; ++q) {
+    XB_REQUIRE(pre_nops[q] >= 0 && post_nops[q] >= 0 && nsel[q] >= 0 && nsel[q] <= nfeat[q % nb], "filter_update_batch: bad counts");
+    for (int k = 0; k < nsel[q]; ++k) XB_REQUIRE(sel[q * F + k] >= 0 && sel[q * F + k] < nfeat[q % nb], "filter_update_batch: sel out of range");
+    first_pre[q] = npre; npre += pre_nops[q];
+    first_post[q] = npost; npost += post_nops[q];
+  }
+  XB_REQUIRE((npre == 0 || pre_ops) && (npost == 0 || post_ops), "filter_update_batch: null edit list");
+  std::vector<EditOp> hops(std::max(1, npre + npost));
+  if (int rc = pack_edits(N, pre_ops, pre_blk, npre, hops.data())) return rc;
+  if (int rc = pack_edits(N, post_ops, post_blk, npost, hops.data() + npre)) return rc;
+  for (int& f : first_post) f += npre;
+  std::vector<CameraParams> hcam(nb);
+  for (size_t b = 0; b < nb; ++b) hcam[b] = cam_from(camera + 11 * b);
+
+  cudaStream_t st = ctx->stream;
+  DevBuf<CameraParams> dcam(nb);
+  DevBuf<double> dX(nb * kPoseDoubles), dgroups(nb * G * kGroupDoubles), dfx(nb * F * 3), dfxp(nb * F * 2), dR(nb), dP(nb * NN), derr(nb * N),
+      dmh(nb * F), ddiag(nb * N), dHP(nb * Mmax * N), dKt(nb * Mmax * N);
+  DevBuf<int> dfref(nb * F), dfsind(nb * F), dnfeat(nb), dsel(npass * nb * F), dnsel(npass * nb), dfirst(4 * npass * nb);
+  DevBuf<FeatJac> djac(nb * F);
+  DevBuf<EditOp> dops(hops.size());
+  XB_REQUIRE(dcam.ok() && dX.ok() && dgroups.ok() && dfx.ok() && dfxp.ok() && dR.ok() && dP.ok() && derr.ok() && dmh.ok() && ddiag.ok() && dHP.ok() &&
+                 dKt.ok() && dfref.ok() && dfsind.ok() && dnfeat.ok() && dsel.ok() && dnsel.ok() && dfirst.ok() && djac.ok() && dops.ok(),
+             "cudaMalloc failed");
+  const bool tensor = (flags & XIVO_UPDATE_TF32X3) != 0, full_j = (flags & XIVO_UPDATE_FULL_J) != 0;
+  const bool v1 = getenv("XIVO_TC_V1") && getenv("XIVO_TC_V1")[0] == '1';
+  TcOperands tc;
+  DevBuf<uint32_t> dKt32, dHP32;
+  if (tensor && !v1) {  // as Batch: allocated and zeroed once; each update rewrites only the k-blocks its M covers
+    const size_t words = tc_operand_words(N, Mmax, batch);
+    dKt32.alloc(words); dHP32.alloc(words);
+    XB_REQUIRE(dKt32.ok() && dHP32.ok(), "cudaMalloc failed");
+    XB_CUDA(cudaMemsetAsync(dKt32.p, 0, words * 4, st));
+    XB_CUDA(cudaMemsetAsync(dHP32.p, 0, words * 4, st));
+    if (int rc = tc_operands_init(&tc, N, Mmax, batch, dKt32.p, dHP32.p)) return rc;
+  }
+  // [pre nops | pre first | post nops | post first], each npass x batch
+  std::vector<int> hfirst(4 * npass * nb);
+  for (size_t q = 0; q < npass * nb; ++q) {
+    hfirst[q] = pre_nops[q]; hfirst[npass * nb + q] = first_pre[q];
+    hfirst[2 * npass * nb + q] = post_nops[q]; hfirst[3 * npass * nb + q] = first_post[q];
+  }
+  XB_CUDA(cudaMemcpyAsync(dcam.p, hcam.data(), sizeof(CameraParams) * nb, cudaMemcpyHostToDevice, st));
+  XB_CUDA(cudaMemcpyAsync(dX.p, X24, sizeof(double) * nb * kPoseDoubles, cudaMemcpyHostToDevice, st));
+  XB_CUDA(cudaMemcpyAsync(dgroups.p, groups, sizeof(double) * nb * G * kGroupDoubles, cudaMemcpyHostToDevice, st));
+  XB_CUDA(cudaMemcpyAsync(dfx.p, feat_x, sizeof(double) * nb * F * 3, cudaMemcpyHostToDevice, st));
+  XB_CUDA(cudaMemcpyAsync(dfxp.p, feat_xp, sizeof(double) * nb * F * 2, cudaMemcpyHostToDevice, st));
+  XB_CUDA(cudaMemcpyAsync(dfref.p, feat_ref, sizeof(int) * nb * F, cudaMemcpyHostToDevice, st));
+  XB_CUDA(cudaMemcpyAsync(dfsind.p, feat_sind, sizeof(int) * nb * F, cudaMemcpyHostToDevice, st));
+  XB_CUDA(cudaMemcpyAsync(dnfeat.p, nfeat, sizeof(int) * nb, cudaMemcpyHostToDevice, st));
+  XB_CUDA(cudaMemcpyAsync(dR.p, Rmeas, sizeof(double) * nb, cudaMemcpyHostToDevice, st));
+  XB_CUDA(cudaMemcpyAsync(dP.p, P, sizeof(double) * nb * NN, cudaMemcpyHostToDevice, st));
+  XB_CUDA(cudaMemcpyAsync(dsel.p, sel, sizeof(int) * npass * nb * F, cudaMemcpyHostToDevice, st));
+  XB_CUDA(cudaMemcpyAsync(dnsel.p, nsel, sizeof(int) * npass * nb, cudaMemcpyHostToDevice, st));
+  XB_CUDA(cudaMemcpyAsync(dfirst.p, hfirst.data(), sizeof(int) * hfirst.size(), cudaMemcpyHostToDevice, st));
+  XB_CUDA(cudaMemcpyAsync(dops.p, hops.data(), sizeof(EditOp) * hops.size(), cudaMemcpyHostToDevice, st));
+  XB_CUDA(cudaMemsetAsync(dmh.p, 0, sizeof(double) * nb * F, st));  // the gate writes features < nfeat only
+  for (int p = 0; p < npass; ++p) {
+    const size_t q = (size_t)p * nb;
+    const int* pre_n = dfirst.p + q;
+    const int* pre_f = dfirst.p + npass * nb + q;
+    const int* post_n = dfirst.p + 2 * npass * nb + q;
+    const int* post_f = dfirst.p + 3 * npass * nb + q;
+    int rc = launch_jacobian_gate(st, lay, dcam.p, dX.p, dgroups.p, dfx.p, dfxp.p, dfref.p, dfsind.p, dnfeat.p, dP.p, dR.p, djac.p, nullptr, dmh.p,
+                                  batch, dops.p, pre_f, pre_n, ddiag.p);
+    if (rc) return rc;
+    rc = launch_ekf_update(st, lay, djac.p, dsel.p + q * F, dnsel.p + q, dR.p, dP.p, derr.p, dHP.p, dKt.p, nullptr, batch, tensor ? 1 : 0, dops.p,
+                           post_f, post_n, tensor && !v1 ? &tc : nullptr, full_j ? 1 : 0);
+    if (rc) return rc;
+    g_launches += 3;
+    XB_CUDA(cudaMemcpyAsync(P_out + q * NN, dP.p, sizeof(double) * nb * NN, cudaMemcpyDeviceToHost, st));
+    XB_CUDA(cudaMemcpyAsync(err + q * N, derr.p, sizeof(double) * nb * N, cudaMemcpyDeviceToHost, st));
+    XB_CUDA(cudaMemcpyAsync(mh + q * F, dmh.p, sizeof(double) * nb * F, cudaMemcpyDeviceToHost, st));
+    XB_CUDA(cudaMemcpyAsync(diag + q * N, ddiag.p, sizeof(double) * nb * N, cudaMemcpyDeviceToHost, st));
+  }
+  XB_CUDA(cudaStreamSynchronize(st));
+  if (tensor) XB_REQUIRE(ekf_cov_tc_fault(st) == 0, "filter_update_batch: the tensor-core downdate timed out waiting for its MMAs");
+  return XIVO_OK;
+}
+
 int xivo_subfilter_batch(xivo_ctx* ctx, const double* camera, const double* X24, int n, const double* x, const double* P33,
                          const double* xp, const double* ref, const double* outlier_counter, double Rtri, double mh_thresh,
                          double* x_out, double* P33_out, double* outlier_counter_out) {
