@@ -32,10 +32,7 @@ int xivo_batch_create(xivo_ctx* ctx, const char* cfg_json, int n_seq, int max_gr
 void xivo_batch_destroy(xivo_batch* b);
 int xivo_batch_size(const xivo_batch* b);
 int xivo_batch_state_dim(const xivo_batch* b); /* kFullSize = 23 + 6 G + 3 F */
-/* Lanes: a batch of many sequences is advanced as several independent lock-step sub-batches ("lanes") of consecutive sequences, each
- * driven by its own library thread, so that the host phases of one lane overlap the GPU phases of the others (the sequences are
- * independent, results do not depend on the lane count).  Count: "lanes" in the config JSON, else the XIVO_LANES environment
- * variable, else one per ~24 sequences.  All entry points keep batch-wide sequence indices. */
+/* Kept for ABI compatibility: always 1 for a valid handle (0 for NULL).  A config with "lanes" > 1 is refused at creation. */
 int xivo_batch_lanes(const xivo_batch* b);
 
 /* Estimator::InertialMeas (src/estimator.cpp:1036-1046), one sample per sequence.

@@ -21,7 +21,6 @@ CFG = os.path.join(ROOT, "xivo_b200", "cfg")
 pytestmark = pytest.mark.gpu
 
 N_STREAMS, N_SEQ, DURATION, G, F = 8, 64, 2.0, 4, 14
-_STREAM_CACHE = {}  # the oracle runs once per session, both parametrisations compare against it
 
 
 def _oracle_stream(seed):
@@ -50,29 +49,22 @@ def _oracle_streams(n, tmp):
     import pickle
     import subprocess
 
-    if n in _STREAM_CACHE:
-        return _STREAM_CACHE[n]
     procs = [subprocess.Popen([sys.executable, os.path.abspath(__file__), str(s), os.path.join(tmp, f"stream{s}.pkl")]) for s in range(n)]
     for p in procs:
         assert p.wait() == 0
-    _STREAM_CACHE[n] = [pickle.load(open(os.path.join(tmp, f"stream{s}.pkl"), "rb")) for s in range(n)]
-    return _STREAM_CACHE[n]
+    return [pickle.load(open(os.path.join(tmp, f"stream{s}.pkl"), "rb")) for s in range(n)]
 
 
-@pytest.mark.parametrize("lanes", [0, 3])
-def test_bench_workload_640x480_150_features_batch_of_64_through_batch_step(tmp_path, lanes):
-    """lanes = 0: one lock-step batch on the shared worker pool (the default and the bench mode); lanes = 3: the same handle split into three
-    independent lanes with a library thread each (`"lanes"` in the config)."""
+def test_bench_workload_640x480_150_features_batch_of_64_through_batch_step(tmp_path):
+    """One lock-step batch on the shared worker pool, driven as bench.py drives each of its batches."""
     from xivo_b200 import pyxivo, sim
 
     streams = _oracle_streams(N_STREAMS, str(tmp_path))
     cfg = sim.load_cfg(os.path.join(CFG, "vio_640x480.json"))
-    if lanes:
-        cfg["lanes"] = lanes
     assert cfg["tracker_cfg"]["num_features_max"] == 150 and cfg["camera_cfg"]["rows"] == 480 and cfg["camera_cfg"]["cols"] == 640
     seq_stream = [(5 * s + 3) % N_STREAMS for s in range(N_SEQ)]  # replicas of a stream are scattered over the batch
     b = pyxivo.Batch(cfg, n_seq=N_SEQ, max_groups=G, max_features=F)
-    assert b.N == 89 and b.lanes == max(1, lanes)
+    assert b.N == 89 and b.lanes == 1
     nframes = len(streams[0]["frames"])
     assert nframes >= 40
     k0 = 0
@@ -102,6 +94,16 @@ def test_bench_workload_640x480_150_features_batch_of_64_through_batch_step(tmp_
     c = b.counters(0)
     assert c["MeasurementUpdateInitialized"] == 1 and c["num_instate_features"] >= 8 and c["error"] == 0
     b.close()
+
+
+def test_config_with_several_lanes_is_refused_at_creation():
+    """A handle is one lock-step batch: "lanes" > 1 in the config fails at creation with a message that names the key."""
+    from xivo_b200 import pyxivo, sim
+    from xivo_b200.capi import XivoError
+
+    cfg = sim.load_cfg(os.path.join(CFG, "vio_640x480.json"))
+    with pytest.raises(XivoError, match="lanes"):
+        pyxivo.Batch(dict(cfg, lanes=3), n_seq=4, max_groups=G, max_features=F)
 
 
 TRACKER_ONLY_512 = {  # the reference's cfg/tumvi_tracker_only_cam0.json:9-56 with SURVEY.md §8d's overrides for configs[0]

@@ -5,13 +5,10 @@
 #include <algorithm>
 #include <atomic>
 #include <chrono>
-#include <condition_variable>
 #include <cstring>
 #include <deque>
-#include <functional>
 #include <mutex>
 #include <stdexcept>
-#include <thread>
 
 #include "../../include/xivo_b200_estimator.h"
 #include "ctx.h"
@@ -161,51 +158,9 @@ struct StreamTicket {
   bool reached(unsigned t) const { return (int)(*reinterpret_cast<volatile unsigned*>(h) - t) >= 0; }
 };
 
-// CPU tokens: with more lane threads than CPUs in the quota, at most `count` of them run host code at a time; a lane hands its token
-// back while it sleeps on a CUDA event.  (Exceeding a cgroup CPU quota stalls every thread of the process for the rest of the period.)
-class CpuTokens {
- public:
-  static CpuTokens& get() {
-    static CpuTokens t;
-    return t;
-  }
-  void acquire() {
-    std::unique_lock<std::mutex> lk(mu_);
-    cv_.wait(lk, [&] { return avail_ > 0; });
-    --avail_;
-  }
-  void release() {
-    {
-      std::lock_guard<std::mutex> lk(mu_);
-      ++avail_;
-    }
-    cv_.notify_one();
-  }
-  int count() const { return count_; }
-
- private:
-  CpuTokens() {
-    const char* e = getenv("XIVO_CPU_TOKENS");
-    int n = e && *e ? atoi(e) : 0;
-    if (n <= 0) {
-      const char* lw = getenv("LOCAL_WORLD_SIZE");
-      const int local_world = std::max(1, lw && *lw ? atoi(lw) : 1);
-      n = std::max(1, host_cpu_budget() / local_world - 1);  // one CPU stays with the caller / CUDA's helper threads
-    }
-    count_ = avail_ = n;
-  }
-  std::mutex mu_;
-  std::condition_variable cv_;
-  int avail_ = 1, count_ = 1;
-};
-
 class Batch {
  public:
-  // lane mode: this batch is one lane of a multi-lane xivo_batch and is driven by its own thread; its per-sequence host code runs
-  // inline on that thread and GPU waits sleep on a blocking event with the CPU token handed back
-  bool lane_mode = false;
-  cudaStream_t st1 = nullptr;  // image-tracker stream: the context's stream for lane 0, an own one otherwise
-  bool own_st1 = false;
+  cudaStream_t st1 = nullptr;  // image-tracker stream: the context's stream
   // Per-sequence host logic is independent across sequences: run it on the process-wide worker pool
   // (workpool.h).  CUDA calls stay on the calling thread.
   // An exception thrown by the host state machine (std::out_of_range of a container lookup, std::bad_alloc) must neither reach a
@@ -220,14 +175,6 @@ class Batch {
   }
   template <typename Fn>
   void pfor(const std::vector<int>& idx, Fn fn) {
-    if (lane_mode) {
-      for (int i = 0; i < (int)idx.size(); ++i) {
-        try { fn(idx[i], i); }
-        catch (const std::exception& ex) { pfor_record(ex.what()); }
-        catch (...) { pfor_record("unknown exception"); }
-      }
-      return;
-    }
     WorkPool::get().pfor((int)idx.size(), [&](int i) {
       try { fn(idx[i], i); }
       catch (const std::exception& ex) { pfor_record(ex.what()); }
@@ -278,7 +225,6 @@ class Batch {
   // pushed, so its copy overlaps the tracking of the frame released now.  ring_ev[slot] orders the two.
   cudaStream_t st_copy = nullptr;
   std::vector<cudaEvent_t> ring_ev;
-  cudaEvent_t wait_ev = nullptr;
   // tracker device state (allocated at the first image)
   bool img_ready = false;
   int rows = 0, cols = 0, cn = 0, ring_n = 0, max_pts = 0, max_kp = 0;
@@ -324,16 +270,12 @@ class Batch {
   // every table of the tracker phase lives in ONE blob: [inputs | pts1 (in/out) | outputs], so the phase costs one H2D and one D2H call
   Mirror<unsigned char> tt;
   size_t tt_up_bytes = 0, tt_down_off = 0, tt_down_bytes = 0;
-  std::string err;
 
-  Batch(xivo_ctx* c, const Json& cfg, int nseq, EkfLayout l, bool tracker_only, int lane = 0, bool lanes = false) : ctx(c), B(nseq), lay(l) {
+  Batch(xivo_ctx* c, const Json& cfg, int nseq, EkfLayout l, bool tracker_only) : ctx(c), B(nseq), lay(l) {
     N = lay.N();
-    lane_mode = lanes;
-    if (lane == 0) st1 = ctx->stream;
-    else { cudaStreamCreateWithFlags(&st1, cudaStreamNonBlocking); own_st1 = true; }
+    st1 = ctx->stream;
     cudaStreamCreateWithFlags(&st2, cudaStreamNonBlocking);
     cudaStreamCreateWithFlags(&st_copy, cudaStreamNonBlocking);
-    cudaEventCreateWithFlags(&wait_ev, cudaEventDisableTiming | (lane_mode ? cudaEventBlockingSync : 0));
     for (int b = 0; b < B; ++b) {
       est.emplace_back(new Estimator(cfg, lay, tracker_only));
       est.back()->compact_records = true;  // imu_cov_propagate rebuilds the intermediate Runge-Kutta stages itself
@@ -438,9 +380,7 @@ class Batch {
   }
   ~Batch() {
     cudaStreamSynchronize(st1);
-    if (own_st1) cudaStreamDestroy(st1);
     if (st2) { cudaStreamSynchronize(st2); cudaStreamDestroy(st2); }
-    if (wait_ev) cudaEventDestroy(wait_ev);
     if (st_copy) { cudaStreamSynchronize(st_copy); cudaStreamDestroy(st_copy); }
     for (cudaEvent_t e : ring_ev) cudaEventDestroy(e);
     for (void* p : {(void*)dP, (void*)dHP, (void*)dKt, (void*)dErr, (void*)dJac, (void*)dRing, (void*)dPyr, (void*)dKt32, (void*)dHP32, (void*)dP0})
@@ -455,7 +395,6 @@ class Batch {
   }
 
   int fail(int code, const std::string& m) {
-    err = m;
     set_error("%s", m.c_str());
     return code;
   }
@@ -563,15 +502,6 @@ class Batch {
   // host memory (StreamTicket); while it is pending the driver executes items of whatever host jobs the other batches of this process
   // have published.  No CUDA call sits in the loop (a stream query every ~2^16 polls only catches a faulted context).
   int wait(cudaStream_t st) {
-    if (lane_mode) {  // sleep on the event; the CPU goes to a lane that has host work
-      XB_CUDA(cudaEventRecord(wait_ev, st));
-      CpuTokens::get().release();
-      const cudaError_t e = cudaEventSynchronize(wait_ev);
-      CpuTokens::get().acquire();
-      if (e != cudaSuccess) { set_error("CUDA error while waiting: %s", cudaGetErrorString(e)); return XIVO_ERR_CUDA; }
-      if (st == st2) { stg_busy[0] = stg_busy[1] = 0; }
-      return 0;
-    }
     static const bool help = !(getenv("XIVO_HELP") && getenv("XIVO_HELP")[0] == '0');
     StreamTicket& t = st == st2 ? tk2 : tk1;
     const unsigned want = ++t.next;
@@ -1698,7 +1628,7 @@ class Batch {
   // sequence runs ahead through its IMU messages until its heap releases a visual message; those are
   // then processed together, and the loop continues with the remaining messages.
   int ingest_many(std::vector<std::vector<Msg>>& in) {
-    if (!lane_mode) WorkPool::get().pin_driver();
+    WorkPool::get().pin_driver();
     std::vector<int> all(B), vis;
     std::vector<size_t> pos(B, 0);
     std::vector<Msg> popped(B), vmsgs;
@@ -1743,7 +1673,7 @@ class Batch {
 
   // Push one message per sequence, then execute whatever each heap releases (MaintainBuffer).
   int ingest(std::vector<Msg>& in) {
-    if (!lane_mode) WorkPool::get().pin_driver();
+    WorkPool::get().pin_driver();
     std::vector<int> all(B), vis;
     std::vector<Msg> popped(B), vmsgs;
     std::vector<char> has(B, 0);
@@ -1774,104 +1704,24 @@ class Batch {
 }  // namespace xb
 
 using namespace xb;
-// A batch handle = one or more LANES: independent lock-step sub-batches of consecutive sequences, each with its own streams, device
-// state and a persistent driver thread.  The sequences of a batch are independent Markov chains, so a lane never talks to another lane;
-// while one lane sleeps on the GPU another one runs its host phases, which keeps both the CPUs of the quota and the GPU busy without
-// fork-join parallel-for rounds inside a phase.  Lane count: "lanes" in the config, else XIVO_LANES, else 1 (a single lock-step batch
-// driven by the calling thread, its per-sequence host code on the shared worker pool).
-struct xivo_batch {
-  xivo_ctx* ctx = nullptr;
-  int total = 0, per = 0, N = 0;
-  std::vector<std::unique_ptr<Batch>> lanes;
-  std::vector<int> first;  // lane l owns sequences [first[l], first[l + 1])
-  std::vector<std::thread> threads;
-  std::mutex mu;
-  std::condition_variable cv_go, cv_done;
-  const std::function<int(int)>* job = nullptr;
-  unsigned long long gen = 0;
-  int pending = 0;
-  bool stop = false;
-  std::vector<int> rc;
-
-  int lane_of(int seq) const { return std::min((int)lanes.size() - 1, seq / per); }
-  void worker(int l) {
-    cudaSetDevice(ctx->device);
-    unsigned long long seen = 0;
-    for (;;) {
-      const std::function<int(int)>* fn;
-      {
-        std::unique_lock<std::mutex> lk(mu);
-        cv_go.wait(lk, [&] { return stop || gen != seen; });
-        if (stop) return;
-        seen = gen;
-        fn = job;
-      }
-      CpuTokens::get().acquire();
-      int r;
-      try { r = (*fn)(l); }
-      catch (const std::exception& ex) { r = lanes[l]->fail(XIVO_ERR_STATE, std::string("lane threw: ") + ex.what()); }
-      catch (...) { r = lanes[l]->fail(XIVO_ERR_STATE, "lane threw"); }
-      CpuTokens::get().release();
-      {
-        std::lock_guard<std::mutex> lk(mu);
-        rc[l] = r;
-        if (--pending == 0) cv_done.notify_all();
-      }
-    }
-  }
-  // fn(lane) on every lane (concurrently when there are several); first non-zero return code, its message re-published on this thread
-  int run(const std::function<int(int)>& fn) {
-    if (lanes.size() == 1) return fn(0);
-    {
-      std::lock_guard<std::mutex> lk(mu);
-      job = &fn;
-      pending = (int)lanes.size();
-      ++gen;
-    }
-    cv_go.notify_all();
-    {
-      std::unique_lock<std::mutex> lk(mu);
-      cv_done.wait(lk, [&] { return pending == 0; });
-    }
-    for (size_t l = 0; l < lanes.size(); ++l)
-      if (rc[l]) { set_error("%s", lanes[l]->err.c_str()); return rc[l]; }
-    return 0;
-  }
-  ~xivo_batch() {
-    {
-      std::lock_guard<std::mutex> lk(mu);
-      stop = true;
-    }
-    cv_go.notify_all();
-    for (auto& t : threads) t.join();
-  }
+// A batch handle is one lock-step Batch, driven by the thread that calls the C ABI; its per-sequence host code runs on the shared worker
+// pool.  Parallelism across sequences beyond one batch comes from several handles per GPU, each driven by its own caller.
+struct xivo_batch : Batch {
+  using Batch::Batch;
 };
 
-static int choose_lanes(const Json& cfg, int n_seq) {
-  int L = cfg.get("lanes", 0);
-  if (L <= 0) {
-    const char* e = getenv("XIVO_LANES");
-    L = e && *e ? atoi(e) : 0;
+#define BATCH_BEGIN                \
+  if (!b) {                        \
+    set_error("null batch");       \
+    return XIVO_ERR_ARG;           \
+  }                                \
+  Batch& B_ = *b;                  \
+  XB_CUDA(cudaSetDevice(B_.ctx->device));
+#define SEQ_CHECK                                     \
+  if (seq < 0 || seq >= B_.B) {                       \
+    set_error("sequence index %d out of range", seq); \
+    return XIVO_ERR_ARG;                              \
   }
-  if (L <= 0) L = 1;  // several lock-step batch handles on the shared worker pool beat lanes, so lanes are opt-in
-  return std::max(1, std::min(L, n_seq));
-}
-
-#define BATCH_BEGIN                                        \
-  if (!b || b->lanes.empty()) {                            \
-    set_error("null batch");                               \
-    return XIVO_ERR_ARG;                                   \
-  }                                                        \
-  xivo_batch& S_ = *b;                                     \
-  XB_CUDA(cudaSetDevice(S_.ctx->device));
-// maps the batch-wide sequence index to (lane B_, index inside the lane)
-#define SEQ_CHECK                                                  \
-  if (seq < 0 || seq >= S_.total) {                                \
-    set_error("sequence index %d out of range", seq);              \
-    return XIVO_ERR_ARG;                                           \
-  }                                                                \
-  Batch& B_ = *S_.lanes[S_.lane_of(seq)];                          \
-  seq -= S_.first[S_.lane_of(seq)];
 
 extern "C" {
 
@@ -1884,22 +1734,11 @@ int xivo_batch_create(xivo_ctx* ctx, const char* cfg_json, int n_seq, int max_gr
   XB_CUDA(cudaSetDevice(ctx->device));
   try {
     Json cfg = Json::parse(cfg_json);
-    std::unique_ptr<xivo_batch> S(new xivo_batch());
-    S->ctx = ctx;
-    S->total = n_seq;
-    const int L = choose_lanes(cfg, n_seq);
-    S->per = (n_seq + L - 1) / L;
-    for (int l = 0; l * S->per < n_seq; ++l) {
-      const int s0 = l * S->per, n = std::min(S->per, n_seq - s0);
-      S->first.push_back(s0);
-      S->lanes.emplace_back(new Batch(ctx, cfg, n, EkfLayout{max_groups, max_features}, tracker_only != 0, l, L > 1));
+    if (cfg.get("lanes", 0) > 1) {
+      set_error("batch_create: \"lanes\" > 1 is not supported; for more parallelism create several batch handles, each driven by its own thread");
+      return XIVO_ERR_ARG;
     }
-    S->first.push_back(n_seq);
-    S->N = S->lanes[0]->N;
-    S->rc.assign(S->lanes.size(), 0);
-    if (S->lanes.size() > 1)
-      for (size_t l = 0; l < S->lanes.size(); ++l) S->threads.emplace_back([p = S.get(), l] { p->worker((int)l); });
-    *out = S.release();
+    *out = new xivo_batch(ctx, cfg, n_seq, EkfLayout{max_groups, max_features}, tracker_only != 0);
   } catch (const std::exception& e) {
     set_error("batch_create: %s", e.what());
     return XIVO_ERR_ARG;
@@ -1912,52 +1751,44 @@ void xivo_batch_destroy(xivo_batch* b) {
   if (b->ctx) cudaSetDevice(b->ctx->device);
   delete b;
 }
-int xivo_batch_size(const xivo_batch* b) { return b ? b->total : 0; }
+int xivo_batch_size(const xivo_batch* b) { return b ? b->B : 0; }
 int xivo_batch_state_dim(const xivo_batch* b) { return b ? b->N : 0; }
-int xivo_batch_lanes(const xivo_batch* b) { return b ? (int)b->lanes.size() : 0; }
+int xivo_batch_lanes(const xivo_batch* b) { return b ? 1 : 0; }
 
 int xivo_batch_inertial_meas(xivo_batch* b, const uint64_t* ts_ns, const double* gyro, const double* accel) {
   BATCH_BEGIN;
   XB_REQUIRE(ts_ns && gyro && accel, "inertial_meas: null argument");
-  return S_.run([&](int l) {
-    Batch& B_ = *S_.lanes[l];
-    const int s0 = S_.first[l];
-    std::vector<Msg> in(B_.B);
-    for (int s = 0; s < B_.B; ++s) {
-      in[s].ts = ts_ns[s0 + s];
-      in[s].type = 0;
-      memcpy(in[s].gyro, gyro + 3 * (size_t)(s0 + s), 24);
-      memcpy(in[s].accel, accel + 3 * (size_t)(s0 + s), 24);
-    }
-    return B_.ingest(in);
-  });
+  std::vector<Msg> in(B_.B);
+  for (int s = 0; s < B_.B; ++s) {
+    in[s].ts = ts_ns[s];
+    in[s].type = 0;
+    memcpy(in[s].gyro, gyro + 3 * (size_t)s, 24);
+    memcpy(in[s].accel, accel + 3 * (size_t)s, 24);
+  }
+  return B_.ingest(in);
 }
 
 static int visual_meas_impl(xivo_batch* b, const uint64_t* ts_ns, const uint8_t* const* imgs, int rows, int cols, int channels,
                             int tracker_only, bool on_device) {
   BATCH_BEGIN;
   XB_REQUIRE(ts_ns && imgs && rows > 0 && cols > 0, "visual_meas: bad arguments");
-  for (int s = 0; s < S_.total; ++s) XB_REQUIRE(imgs[s], "visual_meas: null image");
-  return S_.run([&](int l) {
-    Batch& B_ = *S_.lanes[l];
-    const int s0 = S_.first[l];
-    if (int rc = B_.ensure_images(rows, cols, channels)) return rc;
-    const size_t ib = (size_t)rows * cols * channels;
-    std::vector<Msg> in(B_.B);
-    std::vector<int> slot_of(B_.B);
-    bool uploaded = false;
-    B_.take_slots(imgs + s0, on_device, slot_of, &uploaded);
-    for (int s = 0; s < B_.B; ++s) {
-      in[s].ts = ts_ns[s0 + s];
-      in[s].type = tracker_only ? 2 : 1;
-      in[s].img_slot = slot_of[s];
-    }
-    if (!uploaded)
-      if (int rc = B_.upload_frames(imgs + s0, slot_of, on_device, ib)) return rc;
-    const int rc = B_.ingest(in);
-    const int rc2 = B_.ingest_done(slot_of);
-    return rc ? rc : rc2;
-  });
+  for (int s = 0; s < B_.B; ++s) XB_REQUIRE(imgs[s], "visual_meas: null image");
+  if (int rc = B_.ensure_images(rows, cols, channels)) return rc;
+  const size_t ib = (size_t)rows * cols * channels;
+  std::vector<Msg> in(B_.B);
+  std::vector<int> slot_of(B_.B);
+  bool uploaded = false;
+  B_.take_slots(imgs, on_device, slot_of, &uploaded);
+  for (int s = 0; s < B_.B; ++s) {
+    in[s].ts = ts_ns[s];
+    in[s].type = tracker_only ? 2 : 1;
+    in[s].img_slot = slot_of[s];
+  }
+  if (!uploaded)
+    if (int rc = B_.upload_frames(imgs, slot_of, on_device, ib)) return rc;
+  const int rc = B_.ingest(in);
+  const int rc2 = B_.ingest_done(slot_of);
+  return rc ? rc : rc2;
 }
 
 int xivo_batch_visual_meas(xivo_batch* b, const uint64_t* ts_ns, const uint8_t* const* imgs, int rows, int cols, int channels,
@@ -1972,53 +1803,46 @@ int xivo_batch_step(xivo_batch* b, int n_imu, const uint64_t* imu_ts, const doub
                     const uint8_t* const* imgs, int rows, int cols, int channels, int on_device) {
   BATCH_BEGIN;
   XB_REQUIRE(n_imu >= 0 && frame_ts && imgs && (n_imu == 0 || (imu_ts && gyro && accel)), "batch_step: bad arguments");
-  const int nb = S_.total;  // the IMU arrays are (n_imu, nb[, 3]) over ALL sequences of the batch
+  const int nb = B_.B;  // the IMU arrays are (n_imu, nb[, 3])
   for (int s = 0; s < nb; ++s) XB_REQUIRE(imgs[s], "batch_step: null image");
   HostScope hst("ingest_many_total");
-  return S_.run([&](int l) {
-    Batch& B_ = *S_.lanes[l];
-    const int s0 = S_.first[l];
-    if (int rc = B_.ensure_images(rows, cols, channels)) return rc;
-    const size_t ib = (size_t)rows * cols * channels;
-    std::vector<std::vector<Msg>> in(B_.B);
-    std::vector<int> slot_of(B_.B);
-    bool uploaded = false;
-    B_.take_slots(imgs + s0, on_device != 0, slot_of, &uploaded);
-    {
-      HostScope hm("marshal");
-      for (int s = 0; s < B_.B; ++s) {
-        in[s].resize(n_imu + 1);
-        for (int k = 0; k < n_imu; ++k) {
-          Msg& m = in[s][k];
-          const size_t o = (size_t)k * nb + s0 + s;
-          m.ts = imu_ts[o];
-          m.type = 0;
-          memcpy(m.gyro, gyro + o * 3, 24);
-          memcpy(m.accel, accel + o * 3, 24);
-        }
-        Msg& v = in[s][n_imu];
-        v.ts = frame_ts[s0 + s];
-        v.type = 1;
-        v.img_slot = slot_of[s];
+  if (int rc = B_.ensure_images(rows, cols, channels)) return rc;
+  const size_t ib = (size_t)rows * cols * channels;
+  std::vector<std::vector<Msg>> in(nb);
+  std::vector<int> slot_of(nb);
+  bool uploaded = false;
+  B_.take_slots(imgs, on_device != 0, slot_of, &uploaded);
+  {
+    HostScope hm("marshal");
+    for (int s = 0; s < nb; ++s) {
+      in[s].resize(n_imu + 1);
+      for (int k = 0; k < n_imu; ++k) {
+        Msg& m = in[s][k];
+        const size_t o = (size_t)k * nb + s;
+        m.ts = imu_ts[o];
+        m.type = 0;
+        memcpy(m.gyro, gyro + o * 3, 24);
+        memcpy(m.accel, accel + o * 3, 24);
       }
+      Msg& v = in[s][n_imu];
+      v.ts = frame_ts[s];
+      v.type = 1;
+      v.img_slot = slot_of[s];
     }
-    if (!uploaded)
-      if (int rc = B_.upload_frames(imgs + s0, slot_of, on_device != 0, ib)) return rc;
-    const int rc = B_.ingest_many(in);
-    const int rc2 = B_.ingest_done(slot_of);
-    return rc ? rc : rc2;
-  });
+  }
+  if (!uploaded)
+    if (int rc = B_.upload_frames(imgs, slot_of, on_device != 0, ib)) return rc;
+  const int rc = B_.ingest_many(in);
+  const int rc2 = B_.ingest_done(slot_of);
+  return rc ? rc : rc2;
 }
 
 int xivo_batch_prefetch_frames(xivo_batch* b, const uint8_t* const* imgs, int rows, int cols, int channels) {
   BATCH_BEGIN;
   XB_REQUIRE(imgs && rows > 0 && cols > 0, "prefetch_frames: bad arguments");
-  for (int s = 0; s < S_.total; ++s) XB_REQUIRE(imgs[s], "prefetch_frames: null image");
-  return S_.run([&](int l) {
-    Batch& B_ = *S_.lanes[l];
-    if (int rc = B_.ensure_images(rows, cols, channels)) return rc;
-    return B_.prefetch_frames(imgs + S_.first[l], (size_t)rows * cols * channels);
-  });
+  for (int s = 0; s < B_.B; ++s) XB_REQUIRE(imgs[s], "prefetch_frames: null image");
+  if (int rc = B_.ensure_images(rows, cols, channels)) return rc;
+  return B_.prefetch_frames(imgs, (size_t)rows * cols * channels);
 }
 
 int xivo_set_frame_ingest(int mode) {
@@ -2043,18 +1867,14 @@ int xivo_batch_visual_meas_pointcloud(xivo_batch* b, const uint64_t* ts_ns, cons
                                       const double* const* xp_depth, int tracker_only) {
   BATCH_BEGIN;
   XB_REQUIRE(ts_ns && n_pts && ids && xp_depth, "visual_meas_pointcloud: null argument");
-  return S_.run([&](int l) {
-    Batch& B_ = *S_.lanes[l];
-    const int s0 = S_.first[l];
-    std::vector<Msg> in(B_.B);
-    for (int s = 0; s < B_.B; ++s) {
-      in[s].ts = ts_ns[s0 + s];
-      in[s].type = tracker_only ? 4 : 3;
-      in[s].ids.assign(ids[s0 + s], ids[s0 + s] + n_pts[s0 + s]);
-      in[s].xp_depth.assign(xp_depth[s0 + s], xp_depth[s0 + s] + 3 * (size_t)n_pts[s0 + s]);
-    }
-    return B_.ingest(in);
-  });
+  std::vector<Msg> in(B_.B);
+  for (int s = 0; s < B_.B; ++s) {
+    in[s].ts = ts_ns[s];
+    in[s].type = tracker_only ? 4 : 3;
+    in[s].ids.assign(ids[s], ids[s] + n_pts[s]);
+    in[s].xp_depth.assign(xp_depth[s], xp_depth[s] + 3 * (size_t)n_pts[s]);
+  }
+  return B_.ingest(in);
 }
 
 static void put34(const SE3h& g, double* out) {
@@ -2268,14 +2088,12 @@ int xivo_scale_init_velocity(xivo_batch* b, int seq, double scale) {  // Estimat
 
 int xivo_init_with_sim_depths(xivo_batch* b) {
   BATCH_BEGIN;
-  for (auto& lane : S_.lanes)
-    for (auto& e : lane->est) e->sim_initialize_depths = true;
+  for (auto& e : B_.est) e->sim_initialize_depths = true;
   return 0;
 }
 const char* xivo_batch_error(xivo_batch* b, int seq) {
-  if (!b || b->lanes.empty() || seq < 0 || seq >= b->total) return "";
-  const int l = b->lane_of(seq);
-  return b->lanes[l]->est[seq - b->first[l]]->error_msg.c_str();
+  if (!b || seq < 0 || seq >= b->B) return "";
+  return b->est[seq]->error_msg.c_str();
 }
 
 }  // extern "C"

@@ -58,7 +58,7 @@ class Batch:
         self.n = n_seq
         self.G, self.F = max_groups, max_features
         self.N = L.xivo_batch_state_dim(self._h)
-        self.lanes = L.xivo_batch_lanes(self._h)  # independent lock-step sub-batches, one library thread each (include/xivo_b200_estimator.h)
+        self.lanes = L.xivo_batch_lanes(self._h)  # always 1: kept for callers that record it (include/xivo_b200_estimator.h)
         self._keep = None
         cam = self.cfg.get("camera_cfg") if isinstance(self.cfg.get("camera_cfg"), dict) else None
         self._cam_shape = (int(cam["rows"]), int(cam["cols"])) if cam and "rows" in cam and "cols" in cam else None
