@@ -17,9 +17,8 @@ a, b = synth.frame_pair(960, 1280, seed=3, shift=(3, 2))
 xy, sc, n = ctx.fast_detect(a, 10, max_kp=1 << 17)
 p0 = xy[np.lexsort((xy[:, 0], xy[:, 1], -sc))[:20000]].astype(np.float32)
 print("points", len(p0))
-for env in ({"XIVO_LK_GENERIC": "1"}, {"XIVO_LK_PACK": "0"}, {"XIVO_LK_PACK": "1"}):
-    for k in ("XIVO_LK_GENERIC", "XIVO_LK_PACK"):
-        os.environ.pop(k, None)
+for env in ({"XIVO_LK_GENERIC": "1"}, {}):
+    os.environ.pop("XIVO_LK_GENERIC", None)
     os.environ.update(env)
     for _ in range(3):
         ctx.lk_track(a, b, p0, p0 + 1.0)
@@ -30,14 +29,11 @@ for env in ({"XIVO_LK_GENERIC": "1"}, {"XIVO_LK_PACK": "0"}, {"XIVO_LK_PACK": "1
     r = report()
     print(env, {k: round(v["ms"] / v["calls"] * 1000, 1) for k, v in r.items()})
 
-for env in ({"XIVO_FAST_SCALAR": "1"}, {}):
-    os.environ.pop("XIVO_FAST_SCALAR", None)
-    os.environ.update(env)
-    for _ in range(3):
-        ctx.fast_detect(a, 5, max_kp=1 << 18)
-    L.xivo_profile_reset(); L.xivo_profile_enable(1)
-    for _ in range(10):
-        ctx.fast_detect(a, 5, max_kp=1 << 18)
-    L.xivo_profile_enable(0)
-    r = report()
-    print("fast", env, {k: round(v["ms"] / v["calls"] * 1000, 1) for k, v in r.items()})
+for _ in range(3):
+    ctx.fast_detect(a, 5, max_kp=1 << 18)
+L.xivo_profile_reset(); L.xivo_profile_enable(1)
+for _ in range(10):
+    ctx.fast_detect(a, 5, max_kp=1 << 18)
+L.xivo_profile_enable(0)
+r = report()
+print("fast", {k: round(v["ms"] / v["calls"] * 1000, 1) for k, v in r.items()})

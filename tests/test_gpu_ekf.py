@@ -252,10 +252,9 @@ def test_oos_projection_invariants(ctx, k):
 
 
 @pytest.mark.parametrize("method", ["PrinceDormand", "RK4"])
-def test_imu_cov_propagate_matches_oracle(ctx, method, monkeypatch):
+def test_imu_cov_propagate_matches_oracle(ctx, method):
     """Device covariance propagation (from per-stage records) vs the numpy restatement of
-    Propagate + PrinceDormand/RK4 (fp64, 1e-10); both formulations of the kernel (XIVO_IMU_V1=1 selects the first one)
-    and their agreement with each other."""
+    Propagate + PrinceDormand/RK4 (fp64, 1e-10)."""
     rng = np.random.default_rng(7)
     lay = E.Layout(4, 14)
     N = lay.N
@@ -284,7 +283,3 @@ def test_imu_cov_propagate_matches_oracle(ctx, method, monkeypatch):
     Pg = ctx.imu_cov_propagate(P, np.array(rec), g, qimu, qmodel, nst)
     assert np.abs(Pg - Pr).max() <= 1e-10 * np.abs(Pr).max()
     assert np.abs(Pg - Pg.T).max() <= 1e-13 * np.abs(Pg).max()
-    monkeypatch.setenv("XIVO_IMU_V1", "1")
-    P1 = ctx.imu_cov_propagate(P, np.array(rec), g, qimu, qmodel, nst)
-    assert np.abs(P1 - Pr).max() <= 1e-10 * np.abs(Pr).max()
-    assert np.abs(P1 - Pg).max() <= 1e-13 * np.abs(Pr).max()  # same operation order per element; only FMA contraction may differ

@@ -353,18 +353,12 @@ def _imu_problem(N, method, nsub, seed):
 @pytest.mark.gpu
 @pytest.mark.parametrize("N", [23, 299])
 @pytest.mark.parametrize("method,nsub", [("PrinceDormand", 1), ("RK4", 1), ("PrinceDormand", 146), ("RK4", 256)])
-def test_imu_cov_propagate_edges(ctx, N, method, nsub, monkeypatch):
+def test_imu_cov_propagate_edges(ctx, N, method, nsub):
     """N = 23 (no strips) and N = 299 (the strip loop over 276 columns wraps past 256 threads); one sub-step, and a queue at capacity
-    (1022 Prince-Dormand / 1024 RK4 stages, several chunks of the kernel's stage loader); both formulations."""
+    (1022 Prince-Dormand / 1024 RK4 stages, several chunks of the kernel's stage loader)."""
     P, rec, g, qimu, qmodel, nst, Pr = _imu_problem(N, method, nsub, seed=N + nsub)
     d = np.sqrt(np.outer(np.diag(Pr), np.diag(Pr)))
-    results = []
-    for v1 in ("0", "1"):
-        monkeypatch.setenv("XIVO_IMU_V1", v1)
-        Pg = ctx.imu_cov_propagate(P, rec, g, qimu, qmodel, nst)
-        assert np.abs(Pg - Pr).max() <= 1e-10 * np.abs(Pr).max(), v1
-        assert (np.abs(Pg - Pr) / d).max() <= 1e-10, v1
-        assert np.abs(Pg - Pg.T).max() <= 1e-13 * np.abs(Pg).max()
-        results.append(Pg)
-    monkeypatch.delenv("XIVO_IMU_V1", raising=False)
-    assert np.abs(results[0] - results[1]).max() <= 1e-13 * np.abs(Pr).max()
+    Pg = ctx.imu_cov_propagate(P, rec, g, qimu, qmodel, nst)
+    assert np.abs(Pg - Pr).max() <= 1e-10 * np.abs(Pr).max()
+    assert (np.abs(Pg - Pr) / d).max() <= 1e-10
+    assert np.abs(Pg - Pg.T).max() <= 1e-13 * np.abs(Pg).max()

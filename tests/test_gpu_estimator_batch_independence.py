@@ -69,7 +69,6 @@ MODES = {
     "rk4": ({"integration_method": "RK4"}, {}),
     "tf32x3": ({"covariance_update": "tf32x3"}, {}),
     "tf32x3_tc_v1": ({"covariance_update": "tf32x3"}, {"XIVO_TC_V1": "1"}),
-    "imu_v1": ({}, {"XIVO_IMU_V1": "1"}),
     "one_point_ransac": ({"use_1pt_RANSAC": True, "1pt_RANSAC_thresh": 1.5, "sim_outliers": {"fraction": 0.08, "pixels": 2.5}}, {}),
 }
 

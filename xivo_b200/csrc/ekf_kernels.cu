@@ -637,154 +637,21 @@ __device__ __forceinline__ void imu_load_chunk(const ImuStep* __restrict__ stp, 
   }
 }
 
-__global__ void __launch_bounds__(IMU_THREADS) imu_cov_propagate_kernel(int N, double* __restrict__ P, const ImuStep* __restrict__ steps,
-                                                                        const int* __restrict__ first, const int* __restrict__ nsteps,
-                                                                        const ImuConst* __restrict__ cst) {
-  const int b = blockIdx.x, tid = threadIdx.x;
-  if (nsteps[b] == 0) return;
-  __shared__ double sP[529], sP0[529], sA[7][207], sFK[7][207], sSA[207], sAcc[207], sT9[207], sPhi[207], sV[7][9], sCV[9], sGc[23];
-  __shared__ ImuConst c;
-  __shared__ unsigned char sI[529], sJ[529];  // row / column of a flat 23x23 index (no div/mod in the loops)
-  if (tid < (int)(sizeof(ImuConst) / 8)) reinterpret_cast<double*>(&c)[tid] = reinterpret_cast<const double*>(cst + b)[tid];
-  for (int t = tid; t < 529; t += IMU_THREADS) { sI[t] = (unsigned char)(t / 23); sJ[t] = (unsigned char)(t % 23); }
-  double* __restrict__ Pb = P + (size_t)b * N * N;
-  const ImuStep* __restrict__ stp = steps + first[b];
-  for (int t = tid; t < 529; t += IMU_THREADS) sP[t] = Pb[(size_t)(t / 23) * N + t % 23];
-  for (int t = tid; t < 207; t += IMU_THREADS) sPhi[t] = (t / 23 == t % 23) ? 1.0 : 0.0;
-  __syncthreads();
-  const int nst = c.stages_per_step;
-  const int nall = nsteps[b] * nst;  // stages
-  const bool pd = nst == 7;
-  if (tid < 23) {  // state-independent diagonal of G Q G^T
-    double v = 0.0;
-    if (tid < 3) v = c.qimu[tid];
-    else if (tid >= 9 && tid < 12) v = c.qimu[6 + tid - 9];
-    else if (tid >= 12 && tid < 15) v = c.qimu[9 + tid - 12];
-    sGc[tid] = v;
-  }
-  __syncthreads();
-  // Stages are consumed in chunks of IMU_CHUNK (a multiple of both 7 and 4 stages per substep): the non-zero
-  // blocks of F of every stage of the chunk are built in parallel up front (imu_load_chunk), so the serial stage chain below
-  // never waits on global memory or on the stage rotations.
-  extern __shared__ __align__(16) unsigned char imu_dyn[];
-  F9s* sFc = reinterpret_cast<F9s*>(imu_dyn);
-  double* sH = reinterpret_cast<double*>(sFc + IMU_CHUNK);
-  auto load_chunk = [&](int c0) {
-    __syncthreads();  // the previous chunk is no longer read
-    imu_load_chunk(stp, c0, min(IMU_CHUNK, nall - c0), nst, c, sFc, sH, tid);
-    __syncthreads();
-  };
-  const F9s* pf = sFc;
-  auto stage_products = [&](int s, const double* Pin, double h) {
-    // FK[s] = F + (F acc) h  (acc holds sum a FK; unused for s == 0), A[s] = F[0:9,:] Pin, V[s] = R qa R^T
-    for (int t = tid; t < 207; t += IMU_THREADS) {
-      const int i = sI[t], j = sJ[t];
-      const double fd = f9_dense(*pf, i, j);
-      sFK[s][t] = s == 0 ? fd : fd + f9_elem(*pf, sAcc, i, j, true) * h;
-      sA[s][t] = f9_elem(*pf, Pin, i, j, false);
-    }
-    if (tid < 9) {
-      const int i = tid / 3, j = tid - 3 * i;
-      sV[s][tid] = pf->R[3 * i] * c.qimu[3] * pf->R[3 * j] + pf->R[3 * i + 1] * c.qimu[4] * pf->R[3 * j + 1] + pf->R[3 * i + 2] * c.qimu[5] * pf->R[3 * j + 2];
-    }
-    __syncthreads();
-  };
-  // X += w * (strip_sym(S) + sw * gqg_const + V-block CV)
-  auto add_sym = [&](double* dst, const double* base, double sw, double h) {
-    for (int t = tid; t < 529; t += IMU_THREADS) {
-      const int i = sI[t], j = sJ[t];
-      double inc = (i < 9 ? sSA[i * 23 + j] : 0.0) + (j < 9 ? sSA[j * 23 + i] : 0.0);
-      if (i == j) inc += sw * sGc[i];
-      if (i >= 6 && i < 9 && j >= 6 && j < 9) inc += sCV[(i - 6) * 3 + j - 6];
-      dst[t] = base[t] + inc * h;
-    }
-  };
-  for (int base = 0; base + nst <= nall; base += nst) {
-    if (base % IMU_CHUNK == 0) load_chunk(base);
-    pf = sFc + base % IMU_CHUNK;
-    const double henc = sH[base % IMU_CHUNK];
-    const double h = fabs(henc);
-    stage_products(0, sP, h);
-    for (int s = 1; s < nst; ++s) {
-      const double* a = pd ? kApd[s - 1] : kArk[s - 1];
-      double sa = 0;
-      for (int q = 0; q < s; ++q) sa += a[q];
-      for (int t = tid; t < 207; t += IMU_THREADS) {
-        double f = 0, p = 0;
-        for (int q = 0; q < s; ++q) { f += a[q] * sFK[q][t]; p += a[q] * sA[q][t]; }
-        sAcc[t] = f;
-        sSA[t] = p;
-      }
-      if (tid < 9) {
-        double v = 0;
-        for (int q = 0; q < s; ++q) v += a[q] * sV[q][tid];
-        sCV[tid] = v;
-      }
-      __syncthreads();
-      add_sym(sP0, sP, sa, h);
-      __syncthreads();  // sP0 complete
-      pf = sFc + (base + s) % IMU_CHUNK;
-      stage_products(s, sP0, h);
-    }
-    const double* bw = pd ? kBpd : kBrk;
-    double sb = 0;
-    for (int q = 0; q < nst; ++q) sb += bw[q];
-    for (int t = tid; t < 207; t += IMU_THREADS) {
-      double f = 0, p = 0;
-      for (int q = 0; q < nst; ++q) { f += bw[q] * sFK[q][t]; p += bw[q] * sA[q][t]; }
-      sAcc[t] = ((sI[t] == sJ[t]) ? 1.0 : 0.0) + f * h;  // rows 0..8 of I + FK h
-      sSA[t] = p;
-    }
-    if (tid < 9) {
-      double v = 0;
-      for (int q = 0; q < nst; ++q) v += bw[q] * sV[q][tid];
-      sCV[tid] = v;
-    }
-    __syncthreads();
-    add_sym(sP, sP, sb, h);
-    // Phi <- (I + FK h) Phi; rows >= 9 of both factors are identity rows
-    for (int t = tid; t < 207; t += IMU_THREADS) {
-      const int i = sI[t], j = sJ[t];
-      double v = j >= 9 ? sAcc[i * 23 + j] : 0.0;
-#pragma unroll
-      for (int k = 0; k < 9; ++k) v += sAcc[i * 23 + k] * sPhi[k * 23 + j];
-      sT9[t] = v;
-    }
-    __syncthreads();
-    for (int t = tid; t < 207; t += IMU_THREADS) sPhi[t] = sT9[t];
-    if (henc < 0 && tid < 23) sP[tid * 23 + tid] += c.qmodel[tid];  // end of a Propagate call: += Qmodel (diagonal)
-    __syncthreads();
-  }
-  // write back: motion block and strips (rows 0..8 change)
-  for (int t = tid; t < 529; t += IMU_THREADS) Pb[(size_t)sI[t] * N + sJ[t]] = sP[t];
-  for (int j = 23 + tid; j < N; j += IMU_THREADS) {
-    double col[23];
-#pragma unroll
-    for (int k = 0; k < 23; ++k) col[k] = Pb[(size_t)k * N + j];
-#pragma unroll 1
-    for (int i = 0; i < 9; ++i) {
-      double acc = 0.0;
-#pragma unroll
-      for (int k = 0; k < 23; ++k) acc += sPhi[i * 23 + k] * col[k];
-      Pb[(size_t)i * N + j] = acc;
-      Pb[(size_t)j * N + i] = acc;
-    }
-  }
-}
-
-// Second formulation of the same algebra (identical operation order per element): every thread owns fixed elements — a strip
-// thread keeps its FK[q] / A[q] of all stages of the sub-step in registers, a P thread keeps its covariance entries in registers —
-// so the Runge-Kutta combinations need no shared-memory round trip and no index tables, and the stage chain has two barriers per
-// stage (double-buffered Acc / SA / CV) instead of three.  (A formulation with shared-memory index tables spends its issue slots on
-// index arithmetic and its stalls at barriers rather than on DFMA.)
 __device__ __forceinline__ double v_block(const F9s& f, const ImuConst& c, int e) {  // (R diag(qa) R^T)[e / 3][e % 3]
   const int i = e / 3, j = e - 3 * i;
   return f.R[3 * i] * c.qimu[3] * f.R[3 * j] + f.R[3 * i + 1] * c.qimu[4] * f.R[3 * j + 1] + f.R[3 * i + 2] * c.qimu[5] * f.R[3 * j + 2];
 }
 
-__global__ void __launch_bounds__(IMU_THREADS) imu_cov_propagate_v2_kernel(int N, double* __restrict__ P, const ImuStep* __restrict__ steps,
-                                                                           const int* __restrict__ first, const int* __restrict__ nsteps,
-                                                                           const ImuConst* __restrict__ cst) {
+// Covariance propagation over a filter's queued IMU sub-steps, one CTA per filter: the Runge-Kutta (Prince-Dormand or RK4) stage
+// chain of the 23 x 23 motion block, the 9 x 23 strips of Phi = prod (I + FK h), and at the end rows 0..8 of P against the feature
+// columns (P[0:9, 23:N] = Phi P[0:23, 23:N]).  Every thread owns fixed elements: a strip thread keeps its FK[q] / A[q] of all stages
+// of the sub-step in registers, a P thread keeps its covariance entries in registers.  So the Runge-Kutta combinations need no
+// shared-memory round trip and no index tables, and the stage chain has two barriers per stage (double-buffered Acc / SA / CV).
+// (A formulation with shared-memory index tables and three barriers per stage spends its issue slots on index arithmetic and its
+// stalls at barriers rather than on DFMA, and takes 2.2 times as long: DESIGN.md section 4.)
+__global__ void __launch_bounds__(IMU_THREADS) imu_cov_propagate_kernel(int N, double* __restrict__ P, const ImuStep* __restrict__ steps,
+                                                                        const int* __restrict__ first, const int* __restrict__ nsteps,
+                                                                        const ImuConst* __restrict__ cst) {
   const int b = blockIdx.x, tid = threadIdx.x;
   if (nsteps[b] == 0) return;
   __shared__ double sP[529], sP0[529], sAcc[2][207], sSA[2][207], sPhi[2][207], sCV[2][9], sGc[23];
@@ -821,11 +688,14 @@ __global__ void __launch_bounds__(IMU_THREADS) imu_cov_propagate_v2_kernel(int N
     else if (tid >= 12 && tid < 15) v = c.qimu[9 + tid - 12];
     sGc[tid] = v;
   }
+  // Stages are consumed in chunks of IMU_CHUNK (a multiple of both 7 and 4 stages per substep): the non-zero
+  // blocks of F of every stage of the chunk are built in parallel up front (imu_load_chunk), so the serial stage chain below
+  // never waits on global memory or on the stage rotations.
   extern __shared__ __align__(16) unsigned char imu_dyn[];
   F9s* sFc = reinterpret_cast<F9s*>(imu_dyn);
   double* sH = reinterpret_cast<double*>(sFc + IMU_CHUNK);
-  auto load_chunk = [&](int c0) {  // as in the first formulation
-    __syncthreads();
+  auto load_chunk = [&](int c0) {
+    __syncthreads();  // the previous chunk is no longer read
     imu_load_chunk(stp, c0, min(IMU_CHUNK, nall - c0), nst, c, sFc, sH, tid);
     __syncthreads();
   };
@@ -947,7 +817,6 @@ __global__ void __launch_bounds__(IMU_THREADS) imu_cov_propagate_v2_kernel(int N
   }
 }
 
-// XIVO_IMU_V1=1 routes the propagation through the first formulation (parity tests compare the two)
 int launch_imu_cov_propagate(cudaStream_t st, int N, double* P, const ImuStep* steps, const int* first, const int* nsteps,
                              const ImuConst* cst, int batch) {
   ProfScope ps("imu_cov_propagate", st);
@@ -955,12 +824,9 @@ int launch_imu_cov_propagate(cudaStream_t st, int N, double* P, const ImuStep* s
   static bool attr_set = false;
   if (!attr_set) {
     XB_CUDA(cudaFuncSetAttribute(imu_cov_propagate_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)dyn));
-    XB_CUDA(cudaFuncSetAttribute(imu_cov_propagate_v2_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)dyn));
     attr_set = true;
   }
-  const char* e = getenv("XIVO_IMU_V1");
-  if (e && e[0] == '1') imu_cov_propagate_kernel<<<batch, IMU_THREADS, dyn, st>>>(N, P, steps, first, nsteps, cst);
-  else imu_cov_propagate_v2_kernel<<<batch, IMU_THREADS, dyn, st>>>(N, P, steps, first, nsteps, cst);
+  imu_cov_propagate_kernel<<<batch, IMU_THREADS, dyn, st>>>(N, P, steps, first, nsteps, cst);
   XB_CUDA(cudaGetLastError());
   return 0;
 }

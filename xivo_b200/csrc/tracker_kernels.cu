@@ -372,154 +372,22 @@ int launch_build_pyramid(cudaStream_t st, uint8_t* pyr, unsigned long long pyr_s
 
 // ------------------------------------------------------------------------------------------
 // FAST-9/16 + cornerScore + 3x3 non-max suppression (cv::FastFeatureDetector, TYPE_9_16).
-// One CTA = 64x16 output pixels.  Stage (64+8)x(16+8) grey pixels (ring radius 3 + NMS 1),
-// compute the score on (64+2)x(16+2), suppress, append packed keypoints with an atomic
-// cursor.  For 3-channel input the BGR->grey fixed-point conversion (cv2 4.13 15-bit
-// coefficients) is fused into the tile load, so the image is read exactly once from HBM.
+// One CTA = 64x16 output pixels.  Stage (64+12)x(16+8) grey pixels (ring radius 3 + NMS 1,
+// pair-aligned columns), compute the score on (64+4)x(16+2), suppress, append packed keypoints
+// with an atomic cursor.  For 3-channel input the BGR->grey fixed-point conversion (cv2 4.13
+// 15-bit coefficients) is fused into the tile load, so the image is read exactly once from HBM.
 // Output: packed (y<<20 | x<<8 | score); order is arbitrary (host sorts on the composite key).
 // ------------------------------------------------------------------------------------------
 constexpr int FT_TX = 64, FT_TY = 16, FT_THREADS = 256;
-constexpr int FT_RW = FT_TX + 8, FT_RH = FT_TY + 8;  // pixel region
-constexpr int FT_SW = FT_TX + 2, FT_SH = FT_TY + 2;  // score region
+constexpr int FT_RH = FT_TY + 8;  // pixel region rows
+constexpr int FT_SH = FT_TY + 2;  // score region rows
 
-__device__ __forceinline__ int fast_score(const uint8_t (*t)[FT_RW + 4], int rx, int ry, int thr) {
-  // t indexed [row][col] in region coords; (rx, ry) is the centre.  Works on the raw ring values
-  // p[k] (no signed differences): nvcc 12.9 has been seen to fuse max(best, max(mn, -mx)) into a
-  // 3-input VIMNMX and drop the negation (the kernel returned max_k(v - p_k) - 1), so the only
-  // arithmetic here is min/max of plain operands plus two final subtractions.
-  const int v = t[ry][rx];
-  const int lo = v - thr, hi = v + thr;
-  int p[16];
-  p[0] = t[ry + 3][rx];
-  p[4] = t[ry][rx + 3];
-  p[8] = t[ry - 3][rx];
-  p[12] = t[ry][rx - 3];
-  // any 9-arc of the 16-ring contains >= 2 of the 4 compass points
-  const int nb = (p[0] > hi) + (p[4] > hi) + (p[8] > hi) + (p[12] > hi);
-  const int nd = (p[0] < lo) + (p[4] < lo) + (p[8] < lo) + (p[12] < lo);
-  if (nb < 2 && nd < 2) return 0;
-  p[1] = t[ry + 3][rx + 1];
-  p[2] = t[ry + 2][rx + 2];
-  p[3] = t[ry + 1][rx + 3];
-  p[5] = t[ry - 1][rx + 3];
-  p[6] = t[ry - 2][rx + 2];
-  p[7] = t[ry - 3][rx + 1];
-  p[9] = t[ry - 3][rx - 1];
-  p[10] = t[ry - 2][rx - 2];
-  p[11] = t[ry - 1][rx - 3];
-  p[13] = t[ry + 1][rx - 3];
-  p[14] = t[ry + 2][rx - 2];
-  p[15] = t[ry + 3][rx - 1];
-  unsigned mb = 0, md = 0;
-#pragma unroll
-  for (int k = 0; k < 16; ++k) {
-    mb |= (unsigned)(p[k] > hi) << k;
-    md |= (unsigned)(p[k] < lo) << k;
-  }
-  mb |= mb << 16;
-  md |= md << 16;
-  unsigned ab = mb, ad = md;
-#pragma unroll
-  for (int k = 1; k < 9; ++k) {
-    ab &= mb >> k;
-    ad &= md >> k;
-  }
-  if (((ab | ad) & 0xffffu) == 0) return 0;
-  // cornerScore<16>: largest t such that some 9-arc is entirely darker than v - t or entirely
-  // brighter than v + t:  best = max( v - min_arcs(max p) , max_arcs(min p) - v ), score = best - 1.
-  // min / max over the 16 circular 9-arcs by doubling (windows of 2, 4, 8, then +1): 160 min/max instead of 288
-  int mn[16], mx[16], t2n[16], t2x[16];
-#pragma unroll
-  for (int k = 0; k < 16; ++k) {
-    t2n[k] = min(p[k], p[(k + 1) & 15]);
-    t2x[k] = max(p[k], p[(k + 1) & 15]);
-  }
-#pragma unroll
-  for (int k = 0; k < 16; ++k) {
-    mn[k] = min(t2n[k], t2n[(k + 2) & 15]);
-    mx[k] = max(t2x[k], t2x[(k + 2) & 15]);
-  }
-#pragma unroll
-  for (int k = 0; k < 16; ++k) {
-    t2n[k] = min(mn[k], mn[(k + 4) & 15]);
-    t2x[k] = max(mx[k], mx[(k + 4) & 15]);
-  }
-  int arc_max_min = 255, arc_min_max = 0;
-#pragma unroll
-  for (int k = 0; k < 16; ++k) {
-    const int a_mn = min(t2n[k], p[(k + 8) & 15]);
-    const int a_mx = max(t2x[k], p[(k + 8) & 15]);
-    arc_max_min = min(arc_max_min, a_mx);
-    arc_min_max = max(arc_min_max, a_mn);
-  }
-  const int dark = v - arc_max_min, bright = arc_min_max - v;
-  return (dark > bright ? dark : bright) - 1;  // corner  <=>  best > thr
-}
-
-template <int CN>
-__global__ void __launch_bounds__(FT_THREADS) fast_kernel(const uint8_t* __restrict__ img, unsigned long long img_stride,
-                                                          const unsigned long long* __restrict__ seq_off, int rows, int cols,
-                                                          int thr, int nonmax, unsigned* __restrict__ kp_out, int max_kp,
-                                                          int* __restrict__ kp_count, const int* __restrict__ need) {
-  __shared__ uint8_t tile[FT_RH][FT_RW + 4];
-  __shared__ short score[FT_SH][FT_SW + 2];
-  const unsigned long long soff = seq_off ? seq_off[blockIdx.z] : (unsigned long long)blockIdx.z * img_stride;
-  if (soff == ~0ull) return;  // inactive sequence
-  if (need && need[blockIdx.z] <= 0) return;  // device-side decision of the accept kernel: this sequence keeps enough tracks
-  const uint8_t* __restrict__ src = img + soff;
-  const int ox = blockIdx.x * FT_TX, oy = blockIdx.y * FT_TY;
-  const int tx = threadIdx.x & 31, ty = threadIdx.x >> 5;  // 32 x 8 thread layout, no integer divisions
-  // region origin in image coordinates
-  const int gx0 = ox - 4, gy0 = oy - 4;
-  for (int ry = ty; ry < FT_RH; ry += 8) {
-    const int gy = gy0 + ry;
-    for (int rx = tx; rx < FT_RW; rx += 32) {
-      const int gx = gx0 + rx;
-      int val = 0;
-      if (gx >= 0 && gx < cols && gy >= 0 && gy < rows) {
-        const uint8_t* p = src + ((size_t)gy * cols + gx) * CN;
-        if (CN == 1) val = p[0];
-        else val = (p[0] * 3735 + p[1] * 19235 + p[2] * 9798 + (1 << 14)) >> 15;
-      }
-      tile[ry][rx] = (uint8_t)val;
-    }
-  }
-  __syncthreads();
-  for (int sy = ty; sy < FT_SH; sy += 8) {
-    const int gy = oy - 1 + sy;
-    for (int sx = tx; sx < FT_SW; sx += 32) {
-      const int gx = ox - 1 + sx;
-      int s = 0;
-      if (gx >= 3 && gx < cols - 3 && gy >= 3 && gy < rows - 3) s = fast_score(tile, sx + 3, sy + 3, thr);
-      score[sy][sx] = (short)s;
-    }
-  }
-  __syncthreads();
-  for (int py = ty; py < FT_TY; py += 8) {
-    const int gy = oy + py;
-    for (int px = tx; px < FT_TX; px += 32) {
-      const int gx = ox + px;
-      if (gx >= cols || gy >= rows) continue;
-      const int s = score[py + 1][px + 1];
-      if (s <= 0) continue;
-      bool keep = true;
-      if (nonmax) {
-        keep = s > score[py][px] && s > score[py][px + 1] && s > score[py][px + 2] && s > score[py + 1][px] &&
-               s > score[py + 1][px + 2] && s > score[py + 2][px] && s > score[py + 2][px + 1] && s > score[py + 2][px + 2];
-      }
-      if (keep) {
-        const int idx = atomicAdd(&kp_count[blockIdx.z], 1);
-        if (idx < max_kp) kp_out[(size_t)blockIdx.z * max_kp + idx] = ((unsigned)gy << 20) | ((unsigned)gx << 8) | (unsigned)s;
-      }
-    }
-  }
-}
-
-// Packed variant: a thread scores two horizontally adjacent pixels at once.  The grey tile is kept as 16-bit
-// values so a pixel pair is one 32-bit word; ring values of the pair are word loads (even column offsets) or a
-// byte-permute of two words (odd offsets); all min/max run on s16x2 pairs (3-input where it helps).  No compass
-// pre-test and no arc bit-mask: the corner decision is "best > thr" on the same cornerScore value, which is what
-// the arc test of the scalar kernel evaluates.  ~70 thread instructions per pixel on textured frames instead of ~400.
+// A thread scores two horizontally adjacent pixels at once.  The grey tile is kept as 16-bit values so a pixel
+// pair is one 32-bit word; ring values of the pair are word loads (even column offsets) or a byte-permute of two
+// words (odd offsets); all min/max run on s16x2 pairs (3-input where it helps).  No compass pre-test and no arc
+// bit-mask: the corner decision is "best > thr" on the cornerScore value, which is what the 9-arc test evaluates
+// (the C oracle, oracle/tracker_oracle.c, decides the same way).  ~70 thread instructions per pixel on textured
+// frames instead of ~400 for one pixel per thread with the arc test.
 constexpr int FP_SW = FT_TX + 4;          // score region width (pairs aligned): image x = ox - 2 + sx
 constexpr int FP_RW = FT_TX + 12;         // tile width: image x = ox - 6 + rx (even origin, ring radius 3 on both sides)
 __device__ __forceinline__ unsigned pk_min(unsigned a, unsigned b) { return __vmins2(a, b); }
@@ -697,12 +565,6 @@ __global__ void __launch_bounds__(FT_THREADS) fast_pair_tma_kernel(const __grid_
   fast_pair_tile(tile, score, ox, oy, rows, cols, thr, nonmax, kp_out, max_kp, kp_count);
 }
 
-// XIVO_FAST_SCALAR=1 routes detection through the one-pixel-per-thread kernel (parity tests compare the two)
-static bool force_scalar_fast() {
-  const char* e = getenv("XIVO_FAST_SCALAR");
-  return e && e[0] == '1';
-}
-
 int make_fast_tensor_map(CUtensorMap* out, const uint8_t* base, int rows, int cols, unsigned long long img_stride, unsigned long long n_img) {
   return make_pyr_tensor_map(out, base, rows, cols, img_stride, n_img, FTM_BOXW, FT_RH);
 }
@@ -715,11 +577,8 @@ int launch_fast_detect(cudaStream_t st, const uint8_t* img, unsigned long long i
   if (!count_is_zero) XB_CUDA(cudaMemsetAsync(kp_count, 0, sizeof(int) * batch, st));
   ProfScope ps("fast_detect", st);
   dim3 grid((cols + FT_TX - 1) / FT_TX, (rows + FT_TY - 1) / FT_TY, batch);
-  if (tma_map && cn == 1 && tma_img_stride && !force_scalar_fast()) {
+  if (tma_map && cn == 1 && tma_img_stride) {
     fast_pair_tma_kernel<<<grid, FT_THREADS, 0, st>>>(*tma_map, tma_img_stride, seq_off, rows, cols, thr, nonmax, kp_out, max_kp, kp_count, need);
-  } else if (force_scalar_fast()) {
-    if (cn == 1) fast_kernel<1><<<grid, FT_THREADS, 0, st>>>(img, img_stride, seq_off, rows, cols, thr, nonmax, kp_out, max_kp, kp_count, need);
-    else fast_kernel<3><<<grid, FT_THREADS, 0, st>>>(img, img_stride, seq_off, rows, cols, thr, nonmax, kp_out, max_kp, kp_count, need);
   } else {
     if (cn == 1) fast_pair_kernel<1><<<grid, FT_THREADS, 0, st>>>(img, img_stride, seq_off, rows, cols, thr, nonmax, kp_out, max_kp, kp_count, need);
     else fast_pair_kernel<3><<<grid, FT_THREADS, 0, st>>>(img, img_stride, seq_off, rows, cols, thr, nonmax, kp_out, max_kp, kp_count, need);
@@ -999,8 +858,8 @@ __global__ void __launch_bounds__(LK_WARPS * 32) lk_kernel(const uint8_t* __rest
 // loads 2 bytes per sample slot (rows y, y+1 of its column) and gets the x+1 neighbours by shuffle,
 // instead of 4 loads + 3 shared-memory reads; no integer divisions remain in the loops.
 // (6 CTAs of 4 warps per SM at 80 registers; a 64-register cap for 8 CTAs spills a few words.)
-template <int WIN, bool PACK>
-__global__ void __launch_bounds__(LK_WARPS * 32, PACK ? 6 : 1) lk_kernel_fast(const uint8_t* __restrict__ prev_pyr, const uint8_t* __restrict__ next_pyr,
+template <int WIN>
+__global__ void __launch_bounds__(LK_WARPS * 32, 6) lk_kernel_fast(const uint8_t* __restrict__ prev_pyr, const uint8_t* __restrict__ next_pyr,
                                                                unsigned long long pyr_stride,
                                                                const unsigned long long* __restrict__ prev_off,
                                                                const unsigned long long* __restrict__ next_off, PyrDesc d,
@@ -1126,8 +985,9 @@ __global__ void __launch_bounds__(LK_WARPS * 32, PACK ? 6 : 1) lk_kernel_fast(co
     }
     __syncwarp();
     // template + structure tensor: slot s of this lane is window pixel (y = 2 s + r, x = c)
-    // PACK: Ix | Iy << 16 in one register (|Ix|, |Iy| <= 4080) to raise occupancy
-    int tI[NS], tX[NS], tY[PACK ? 1 : NS];
+    // Ix | Iy << 16 in one register (|Ix|, |Iy| <= 4080) to raise occupancy: 80 registers -> 6 CTAs/SM, measured 17 % faster than
+    // keeping Ix and Iy in separate registers
+    int tI[NS], tX[NS];
     int pA11 = 0, pA12 = 0, pA22 = 0;  // per-lane partials: <= 8 samples of |Ix|, |Iy| <= 4080 -> < 2^27
 #pragma unroll
     for (int s = 0; s < NS; ++s) {
@@ -1142,8 +1002,7 @@ __global__ void __launch_bounds__(LK_WARPS * 32, PACK ? 6 : 1) lk_kernel_fast(co
         iy = descale(((int)d00 >> 16) * iw00 + ((int)d01 >> 16) * iw01 + ((int)d10 >> 16) * iw10 + ((int)d11 >> 16) * iw11, 14);
       }
       tI[s] = ival;
-      if (PACK) tX[s] = (ix & 0xffff) | (iy << 16);
-      else { tX[s] = ix; tY[s] = iy; }
+      tX[s] = (ix & 0xffff) | (iy << 16);
       pA11 += ix * ix;
       pA12 += ix * iy;
       pA22 += iy * iy;
@@ -1208,13 +1067,8 @@ __global__ void __launch_bounds__(LK_WARPS * 32, PACK ? 6 : 1) lk_kernel_fast(co
 #pragma unroll
       for (int s = 0; s < NS; ++s) {
         const int diff = bilinear(v0[s], v1[s]) - tI[s];
-        if (PACK) {
-          pb1 += diff * (int)(short)(tX[s] & 0xffff);
-          pb2 += diff * (tX[s] >> 16);
-        } else {
-          pb1 += diff * tX[s];
-          pb2 += diff * tY[s];
-        }
+        pb1 += diff * (int)(short)(tX[s] & 0xffff);
+        pb2 += diff * (tX[s] >> 16);
       }
       const long long lb1 = warp_sum_i32_exact(pb1), lb2 = warp_sum_i32_exact(pb2);
       const float b1 = __ll2float_rn(lb1) * FLT_SCALE, b2 = __ll2float_rn(lb2) * FLT_SCALE;
@@ -1266,11 +1120,11 @@ __global__ void __launch_bounds__(LK_WARPS * 32, PACK ? 6 : 1) lk_kernel_fast(co
   }
 }
 
-template <int WIN, bool PACK>
+template <int WIN>
 static void launch_lk_fast(dim3 grid, cudaStream_t st, const uint8_t* prev_pyr, const uint8_t* next_pyr, unsigned long long pyr_stride,
                            const unsigned long long* prev_off, const unsigned long long* next_off, const PyrDesc& d, const float* prev_pts,
                            float* next_pts, uint8_t* status, float* err, const int* npts_dev, const LKParams& prm) {
-  lk_kernel_fast<WIN, PACK><<<grid, LK_WARPS * 32, 0, st>>>(prev_pyr, next_pyr, pyr_stride, prev_off, next_off, d, prev_pts, next_pts, status, err, npts_dev, prm);
+  lk_kernel_fast<WIN><<<grid, LK_WARPS * 32, 0, st>>>(prev_pyr, next_pyr, pyr_stride, prev_off, next_off, d, prev_pts, next_pts, status, err, npts_dev, prm);
 }
 
 // XIVO_LK_GENERIC=1 routes single-channel frames through the generic kernel (parity tests compare the two)
@@ -1305,12 +1159,9 @@ int launch_lk_track(cudaStream_t st, const uint8_t* prev_pyr, const uint8_t* nex
   dim3 grid((max_pts + LK_WARPS - 1) / LK_WARPS, batch);
   ProfScope ps("lk_track", st);
   const bool generic = prm_force_generic_lk();
-  const char* pk = getenv("XIVO_LK_PACK");
-  const bool pack = !(pk && pk[0] == '0');  // default on: 80 registers -> 6 CTAs/SM, measured 17 % faster than the unpacked form
   if (d.cn == 1 && win <= 15 && !generic) {
     switch (win) {
-#define XB_LK_CASE(W) case W: if (pack) launch_lk_fast<W, true>(grid, st, prev_pyr, next_pyr, pyr_stride, prev_off, next_off, d, prev_pts, next_pts, status, err, npts_dev, prm); \
-                           else launch_lk_fast<W, false>(grid, st, prev_pyr, next_pyr, pyr_stride, prev_off, next_off, d, prev_pts, next_pts, status, err, npts_dev, prm); break;
+#define XB_LK_CASE(W) case W: launch_lk_fast<W>(grid, st, prev_pyr, next_pyr, pyr_stride, prev_off, next_off, d, prev_pts, next_pts, status, err, npts_dev, prm); break;
       XB_LK_CASE(3) XB_LK_CASE(5) XB_LK_CASE(7) XB_LK_CASE(9) XB_LK_CASE(11) XB_LK_CASE(13) XB_LK_CASE(15)
 #undef XB_LK_CASE
     }
