@@ -133,7 +133,29 @@ int xivo_get_just_dropped(xivo_batch* b, int seq, int* ids, int max_n, int* n); 
 /* {num_tracker_outlier_rejected, num_tracker_failed_to_track, num_tracker_new_detections, num_oneptransac_rejected} */
 int xivo_get_tracker_counters(xivo_batch* b, int seq, int out[4]);
 int xivo_scale_init_velocity(xivo_batch* b, int seq, double scale); /* Estimator::ScaleInitVelocity: Vsb /= scale */
-int xivo_init_with_sim_depths(xivo_batch* b); /* Estimator::InitWithSimDepths */
+int xivo_init_with_sim_depths(xivo_batch* b); /* Estimator::InitWithSimDepths; a handle-level switch that reset sequences inherit */
+
+/* Sequence `seq` starts over as a freshly created estimator: empty message heap, clocks cleared,
+ * gravity / vision / update not initialised, tracker not initialised, feature and group ids from
+ * their initial values, counters and error zero, its block of P = the initial covariance.
+ * From this call on the sequence is bit-identical to sequence 0 of a new one-sequence handle
+ * (same config, G, F, tracker_only) fed the same messages; every other sequence continues
+ * bit-identically to a run without the call, its queued messages and frames included.
+ * The sequence's pending heap messages are discarded (their frame ring slots become free), and
+ * pending xivo_batch_prefetch_frames uploads are dropped for the whole handle.
+ * cfg_json == NULL: the handle's creation config; otherwise a config of its own, which must agree
+ * with the handle on every batch-wide setting: the layout (G, F) and tracker_only,
+ * "covariance_update", "use_1pt_RANSAC", "subfilter" {"visual_meas_std", "MH_thresh"}, every key of
+ * "tracker_cfg", "camera_cfg" {"rows", "cols"} and "message_buffer_size".  Everything else
+ * (camera model and intrinsics, X incl. Rbc / Tbc, P, Qimu, Qmodel, visual_meas_std, the
+ * integration method, gating and feature-management thresholds, ...) may differ per sequence.
+ * Per-sequence configs from the start: create the handle with any compatible config, then reset
+ * every sequence with its own before the first message.
+ * Returns XIVO_ERR_ARG for a NULL handle, `seq` out of range, a config that does not parse or that
+ * differs in a batch-wide setting (xivo_last_error names the first such key); XIVO_ERR_STATE once an
+ * earlier call on the handle failed (such a call stops mid-frame for every sequence).  A refused
+ * call changes nothing. */
+int xivo_batch_reset_sequence(xivo_batch* b, int seq, const char* cfg_json);
 const char* xivo_batch_error(xivo_batch* b, int seq);
 
 #ifdef __cplusplus

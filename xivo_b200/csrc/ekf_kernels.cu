@@ -547,6 +547,24 @@ int launch_pack_state(cudaStream_t st, int N, const double* P, const double* err
   return 0;
 }
 
+// Initial covariance of filters first .. first + count - 1 (Estimator::Estimator, estimator.cpp:258-302): identity with the filter's own
+// 23 x 23 motion block.  Grid: (column tiles, count); thread = one column of one row chunk, so the stores of a warp are contiguous.
+__global__ void __launch_bounds__(256) cov_init_kernel(int N, double* __restrict__ P, const double* __restrict__ Pmm, int first) {
+  const int b = first + blockIdx.y;
+  const int j = blockIdx.x * 256 + threadIdx.x;
+  if (j >= N) return;
+  double* __restrict__ Pb = P + (size_t)b * N * N;
+  const double* __restrict__ Mb = Pmm + (size_t)b * 529;
+  for (int i = 0; i < N; ++i) Pb[(size_t)i * N + j] = (i < 23 && j < 23) ? Mb[i * 23 + j] : (i == j ? 1.0 : 0.0);
+}
+int launch_cov_init(cudaStream_t st, int N, double* P, const double* Pmm, int first, int count) {
+  if (count <= 0) return 0;
+  ProfScope ps("cov_init", st);
+  cov_init_kernel<<<dim3((N + 255) / 256, count), 256, 0, st>>>(N, P, Pmm, first);
+  XB_CUDA(cudaGetLastError());
+  return 0;
+}
+
 // ------------------------------------------------------------------------------------------
 // IMU covariance propagation: the covariance side of Estimator::Propagate -> PrinceDormand / RK4
 // (/root/reference/src/estimator.cpp:539-704, src/princedormand.cpp:85-221, src/rk4.cpp:35-103).

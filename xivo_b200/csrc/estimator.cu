@@ -217,6 +217,10 @@ class Batch {
   int stg_half = 0;
   unsigned stg_busy[2] = {0, 0};  // st2 ticket after which the half may be refilled (0 = free)
   Mirror<ImuConst> icst;
+  Mirror<double> pmm0;      // B x 23 x 23: initial motion covariance of every filter (cov_init_kernel)
+  Json cfg0;                // the creation config: what a reset sequence gets when it is given none
+  bool sim_depths = false;  // xivo_init_with_sim_depths was called: a reset sequence inherits it
+  unsigned reset_busy = 0;  // st2 ticket after which the host mirrors of the last reset's uploads may be rewritten (0 = free)
   StreamTicket tk1, tk2;    // completion flags of st1 / st2
   // The covariance side (IMU propagation, slot edits, Jacobians, update) runs on its own stream so that it
   // overlaps the image tracker's kernels and host phases, which use ctx->stream.
@@ -271,7 +275,7 @@ class Batch {
   Mirror<unsigned char> tt;
   size_t tt_up_bytes = 0, tt_down_off = 0, tt_down_bytes = 0;
 
-  Batch(xivo_ctx* c, const Json& cfg, int nseq, EkfLayout l, bool tracker_only) : ctx(c), B(nseq), lay(l) {
+  Batch(xivo_ctx* c, const Json& cfg, int nseq, EkfLayout l, bool tracker_only) : ctx(c), B(nseq), lay(l), cfg0(cfg) {
     N = lay.N();
     st1 = ctx->stream;
     cudaStreamCreateWithFlags(&st2, cudaStreamNonBlocking);
@@ -291,7 +295,7 @@ class Batch {
               cudaMalloc(reinterpret_cast<void**>(&dErr), sizeof(double) * B * N) == cudaSuccess &&
               cudaMalloc(reinterpret_cast<void**>(&dJac), sizeof(FeatJac) * B * lay.F) == cudaSuccess;
     ok = ok && cam.alloc(B) && R.alloc(B) && mh.alloc((size_t)B * lay.F + (size_t)B * N) && pack.alloc((size_t)B * (2 * N + 529)) && sub_out.alloc((size_t)B * max_sub) &&
-         icst.alloc(B) && tk1.alloc() && tk2.alloc();
+         icst.alloc(B) && pmm0.alloc((size_t)B * 529) && tk1.alloc() && tk2.alloc();
     if (ok) {  // the per-phase upload blobs and the table views inside them
       struct Carve {
         size_t off = 0;
@@ -353,30 +357,78 @@ class Batch {
            tc_operands_init(&tcops, N, 2 * lay.F, B, dKt32, dHP32) == 0;
     }
     if (!ok) throw std::runtime_error(std::string("device allocation failed: ") + cudaGetErrorString(cudaGetLastError()));
-    // initial covariance: identity with the motion block from the config (estimator.cpp:258-302)
-    std::vector<double> P0((size_t)N * N, 0.0);
-    for (int i = 0; i < N; ++i) P0[(size_t)i * N + i] = 1.0;
-    for (int i = 0; i < 23; ++i)
-      for (int j = 0; j < 23; ++j) P0[(size_t)i * N + j] = est[0]->Pmm[i * 23 + j];
-    for (int b = 0; b < B; ++b) {
-      cudaMemcpy(dP + (size_t)b * N * N, P0.data(), sizeof(double) * N * N, cudaMemcpyHostToDevice);
-      cam.h[b] = est[b]->cam;
-      R.h[b] = est[b]->c.R;
-      {
-        const EstimatorCfg& ec = est[b]->c;
-        ImuConst& ic = icst.h[b];
-        memcpy(ic.g, ec.g.v, 24);
-        for (int i = 0; i < 12; ++i) ic.qimu[i] = ec.Qimu[i * 12 + i];
-        for (int i = 0; i < 23; ++i) ic.qmodel[i] = ec.Qmodel[i * 23 + i];
-        ic.stages_per_step = ec.integration_method == "PrinceDormand" ? 7 : 4;
-        ic.pad = 0;
-      }
-      for (int i = 0; i < N; ++i) est[b]->diagP[i] = P0[(size_t)i * N + i];
-    }
+    for (int b = 0; b < B; ++b) set_filter_tables(b);
     cam.up(st1);
     R.up(st1);
     icst.up(st1);
+    pmm0.up(st1);
+    if (launch_cov_init(st1, N, dP, pmm0.d, 0, B)) throw std::runtime_error(std::string("initial covariance: ") + cudaGetErrorString(cudaGetLastError()));
     cudaStreamSynchronize(st1);
+  }
+  // Host mirrors of sequence b's per-filter device tables (camera, measurement noise, IMU constants, initial motion covariance) from
+  // est[b], and the diagonal of its initial covariance: identity with the motion block from the config (estimator.cpp:258-302).
+  void set_filter_tables(int b) {
+    Estimator& e = *est[b];
+    cam.h[b] = e.cam;
+    R.h[b] = e.c.R;
+    ImuConst& ic = icst.h[b];
+    memcpy(ic.g, e.c.g.v, 24);
+    for (int i = 0; i < 12; ++i) ic.qimu[i] = e.c.Qimu[i * 12 + i];
+    for (int i = 0; i < 23; ++i) ic.qmodel[i] = e.c.Qmodel[i * 23 + i];
+    ic.stages_per_step = e.c.integration_method == "PrinceDormand" ? 7 : 4;
+    ic.pad = 0;
+    memcpy(pmm0.h + (size_t)b * 529, e.Pmm, sizeof(e.Pmm));
+    for (int i = 0; i < N; ++i) e.diagP[i] = i < 23 ? e.Pmm[i * 23 + i] : 1.0;
+  }
+
+  // ---- sequence lifecycle (xivo_batch_reset_sequence) -------------------------------------
+  // Sequence `seq` starts over as a freshly created estimator configured by cfg (null: the handle's creation config); the other
+  // sequences, their heaps and their frames in the ring are untouched.  Refused without any change when an earlier call failed, when
+  // the config does not parse or when it differs from the handle in a batch-wide setting (batch_incompatibility).
+  int reset_sequence(int seq, const Json* cfg) {
+    if (pfor_bad.load()) return fail(XIVO_ERR_STATE, "reset_sequence: an earlier call on this handle failed (" + pfor_msg + "); the handle cannot continue");
+    for (int b = 0; b < B; ++b)
+      if (est[b]->error)
+        return fail(XIVO_ERR_STATE, "reset_sequence: an earlier call on this handle failed (sequence " + std::to_string(b) + ": " + est[b]->error_msg +
+                                        "); the handle cannot continue");
+    std::unique_ptr<Estimator> e;
+    try {
+      e.reset(new Estimator(cfg ? *cfg : cfg0, lay, est[0]->tracker_only));
+    } catch (const std::exception& ex) {
+      return fail(XIVO_ERR_ARG, std::string("reset_sequence: bad config: ") + ex.what());
+    }
+    const std::string key = batch_incompatibility(*est[0], *e);
+    if (!key.empty()) return fail(XIVO_ERR_ARG, "reset_sequence: \"" + key + "\" differs from the handle's; it must be the same for every sequence of a batch");
+    // the host mirrors of the per-filter tables may be rewritten once the uploads of an earlier reset have left them
+    if (reset_busy && !tk2.reached(reset_busy))
+      if (int rc = wait(st2)) return rc;
+    reset_busy = 0;
+    e->compact_records = true;
+    e->sim_initialize_depths = sim_depths;
+    if (img_ready) {  // what ensure_images gives every estimator at the first image
+      e->rows = rows; e->cols = cols;
+      e->mask_stride = (cols + 63) / 64;
+      if (!dev_decide) e->mask.assign((size_t)rows * e->mask_stride, 0);
+      prev_slot[seq] = 0;
+    }
+    est[seq] = std::move(e);  // the old estimator's heap, pending propagation records and edits go with it
+    table_order[seq].clear();
+    if (desc_on) { sorted_kp[seq].clear(); query_feats[seq].clear(); }
+    if (!pref.empty()) {  // pending prefetches are dropped as take_slots drops them: their slots are handed out again
+      for (int s = 0; s < B; ++s) ring_next[s] = pref.front().slot[s];
+      pref.clear();
+    }
+    set_filter_tables(seq);
+    // Device side on st2, in stream order behind the work already queued for the old sequence (an imu_cov_propagate of a frame the heap
+    // has released reads icst and P), ahead of everything the new one enqueues.
+    XB_CUDA(cam.up(st2, 1, seq));
+    XB_CUDA(R.up(st2, 1, seq));
+    XB_CUDA(icst.up(st2, 1, seq));
+    XB_CUDA(pmm0.up(st2, 529, (size_t)seq * 529));
+    if (int rc = launch_cov_init(st2, N, dP, pmm0.d, seq, 1)) return rc;
+    g_launches += 1;
+    reset_busy = tk2.next + 1;  // the next ticket of st2 lies behind these uploads
+    return 0;
   }
   ~Batch() {
     cudaStreamSynchronize(st1);
@@ -387,7 +439,7 @@ class Batch {
       if (p) cudaFree(p);
     cam.release(); R.release(); mh.release(); pack.release(); sub_out.release(); blobS.release(); blobJ.release(); blobU.release();
     blobI[0].release(); blobI[1].release(); tk1.release(); tk2.release();
-    icst.release(); blobG.release();
+    icst.release(); pmm0.release(); blobG.release();
     lkerr.release(); lkst.release(); kpcount.release();
     kp.release(); tt.release();
     descT.release(); validT.release(); kpxy.release(); nkps.release(); nq.release(); descK.release(); validK.release(); qdesc.release();
@@ -435,8 +487,8 @@ class Batch {
     if (!any) return 0;
     // A queue longer than the per-filter staging capacity (an IMU / vision gap of several hundred ms: the reference integrates any dt,
     // estimator.cpp:539-592) goes down in several launches of whole sub-steps each; the kernel composes per launch.
-    const int sps = std::max(1, icst.h[act[0]].stages_per_step);
-    const int chunk = kMaxStages / sps;  // sub-steps per launch
+    // sub-steps per launch and filter: the integration method (and with it the stages per sub-step) is a per-sequence setting
+    auto chunk = [&](int b) { return kMaxStages / std::max(1, icst.h[b].stages_per_step); };
     std::vector<size_t> cur(B, 0);
     for (;;) {
       const int h = stg_half;
@@ -450,7 +502,7 @@ class Batch {
       bool more = false;
       for (int b : act) {
         Estimator& e = *est[b];
-        const int n = (int)std::min<size_t>((size_t)chunk, e.steps.size() - cur[b]);
+        const int n = (int)std::min<size_t>((size_t)chunk(b), e.steps.size() - cur[b]);
         if (n <= 0) continue;
         stg_first[h].h[b] = total;
         stg_n[h].h[b] = n;
@@ -2089,7 +2141,20 @@ int xivo_scale_init_velocity(xivo_batch* b, int seq, double scale) {  // Estimat
 int xivo_init_with_sim_depths(xivo_batch* b) {
   BATCH_BEGIN;
   for (auto& e : B_.est) e->sim_initialize_depths = true;
+  B_.sim_depths = true;
   return 0;
+}
+int xivo_batch_reset_sequence(xivo_batch* b, int seq, const char* cfg_json) {
+  BATCH_BEGIN; SEQ_CHECK;
+  if (!cfg_json) return B_.reset_sequence(seq, nullptr);
+  Json cfg;
+  try {
+    cfg = Json::parse(cfg_json);
+  } catch (const std::exception& e) {
+    set_error("reset_sequence: config does not parse: %s", e.what());
+    return XIVO_ERR_ARG;
+  }
+  return B_.reset_sequence(seq, &cfg);
 }
 const char* xivo_batch_error(xivo_batch* b, int seq) {
   if (!b || seq < 0 || seq >= b->B) return "";

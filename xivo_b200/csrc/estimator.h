@@ -577,4 +577,8 @@ class Estimator {
   std::vector<GroupRow> instate_group_rows(const double* P) const;
 };
 
+// The first setting that one batch handle needs to be the same for every sequence and that differs between the two estimators,
+// as its config key ("tracker_cfg.KLT.win_size"), or "" when a sequence configured like `b` may join a handle configured like `a`.
+std::string batch_incompatibility(const Estimator& a, const Estimator& b);
+
 }  // namespace xb

@@ -135,6 +135,9 @@ int launch_cov_propagate(cudaStream_t st, int N, double* P, const double* Phi /*
 // [err | Pmm | diag(P)] per filter, 2N+529 doubles each.
 int launch_pack_state(cudaStream_t st, int N, const double* P, const double* err, double* out, int batch);
 
+// P of filters [first, first + count) <- identity with the filter's motion block Pmm[b] (B x 23 x 23) in the top-left corner.
+int launch_cov_init(cudaStream_t st, int N, double* P, const double* Pmm, int first, int count);
+
 // Depth sub-filter, thread per feature (Feature::SubfilterUpdate).
 struct SubfilterIn {
   double x[3], P[9], xp[2], ref[kGroupDoubles], outlier_counter;

@@ -37,17 +37,23 @@ def _resolve_cfg(cfg, base_dir=None) -> str:
     return json.dumps(d)
 
 
+def _cfg_text(cfg, overrides=None) -> str:
+    """_resolve_cfg, then `overrides` merged in (one level deep for nested objects)."""
+    text = _resolve_cfg(cfg)
+    if overrides:
+        d = json.loads(text)
+        for k, v in overrides.items():
+            if isinstance(v, dict) and isinstance(d.get(k), dict):
+                d[k].update(v)
+            else:
+                d[k] = v
+        text = json.dumps(d)
+    return text
+
+
 class Batch:
     def __init__(self, cfg, n_seq=1, max_groups=15, max_features=30, tracker_only=False, device=0, ctx=None, overrides=None):
-        text = _resolve_cfg(cfg)
-        if overrides:
-            d = json.loads(text)
-            for k, v in overrides.items():
-                if isinstance(v, dict) and isinstance(d.get(k), dict):
-                    d[k].update(v)
-                else:
-                    d[k] = v
-            text = json.dumps(d)
+        text = _cfg_text(cfg, overrides)
         self.cfg = json.loads(text)
         self._own_ctx = ctx is None
         self.ctx = ctx or capi.Context(device)
@@ -153,6 +159,15 @@ class Batch:
 
     def init_with_sim_depths(self):
         _check(capi.lib().xivo_init_with_sim_depths(self._h), "xivo_init_with_sim_depths")
+
+    def reset_sequence(self, seq, cfg=None, overrides=None):
+        """Sequence `seq` starts over as a new estimator (xivo_batch_reset_sequence): with the handle's creation config when cfg and
+        overrides are None, else with `cfg` (default: the creation config) plus `overrides`, resolved as in __init__.  The config must
+        agree with the handle on the batch-wide settings; a refusal raises XivoError and leaves the handle unchanged."""
+        text = None
+        if cfg is not None or overrides:
+            text = _cfg_text(self.cfg if cfg is None else cfg, overrides).encode()
+        _check(capi.lib().xivo_batch_reset_sequence(self._h, int(seq), text), "xivo_batch_reset_sequence")
 
     # ---- read-back ----------------------------------------------------------------------
     def _g(self, fn, seq):
