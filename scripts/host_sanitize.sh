@@ -1,6 +1,7 @@
 # usage: bash scripts/host_sanitize.sh  (CPU only) -- the product's host state machine under AddressSanitizer + UBSan:
-# tests/cpp/host_harness.cpp (= csrc/estimator.h + estimator_host.cpp.inc + triangulate.h + homography.h) is compiled with
-# -fsanitize=address,undefined and driven by the host-logic and twin tests (whole sequences, every decision checked against the oracle).
+# tests/cpp/host_harness.cpp (= csrc/estimator.h + estimator_host.cpp.inc + tracker_host.cpp.inc + triangulate.h + homography.h) is
+# compiled with -fsanitize=address,undefined and driven by the host-logic and twin tests (whole point-cloud and tracker-only image
+# sequences, every decision checked against the oracle).
 set -e
 SO=/tmp/libhost_harness_asan.so
 g++ -std=c++17 -O1 -g -march=x86-64-v3 -fsanitize=address,undefined -fno-omit-frame-pointer -I "${CUDA_HOME:-/usr/local/cuda}/include" -shared -fPIC tests/cpp/host_harness.cpp -o $SO

@@ -1,9 +1,9 @@
 // CPU test harness for the host state machine of the estimator (xivo_b200/csrc/estimator.h +
-// estimator_host.cpp.inc): compiled with g++ (no nvcc, no GPU) into a small shared object that
-// tests/test_host_logic.py drives through ctypes.  Test infrastructure only — nothing here is linked into
-// libxivo_b200.so; the device phases of the pipeline are not emulated, only the host-side pieces that need
-// no kernel output: configuration, message heap, clocks, gravity initialisation, the nominal-state
-// Runge-Kutta chain with its per-stage records (what imu_cov_propagate consumes) and the tracker mask.
+// estimator_host.cpp.inc + tracker_host.cpp.inc): compiled with g++ (no nvcc, no GPU) into a small shared object that
+// tests/test_host_logic.py and tests/test_host_twin.py drive through ctypes.  Test infrastructure only — nothing here is
+// linked into libxivo_b200.so.  No kernel is emulated: the callers supply what the device phases compute (the twin tests
+// take it from the oracle), and the entry points run the host decisions in between — configuration, message heap, clocks,
+// gravity initialisation, the nominal-state Runge-Kutta chain, the filter's update steps and the image tracker.
 #include <chrono>
 #include <cstring>
 #include <string>
@@ -18,6 +18,7 @@ struct HostScope {  // the library's version also feeds the profiler; timing is 
 }  // namespace xb
 
 #include "../../xivo_b200/csrc/estimator_host.cpp.inc"
+#include "../../xivo_b200/csrc/tracker_host.cpp.inc"
 
 namespace {
 std::string g_err;
@@ -252,9 +253,7 @@ const char* hh_error_msg(void* h) { return static_cast<xb::Estimator*>(h)->error
 // tracker mask (tracker.cpp:471-488, :760-774)
 void hh_mask_init(void* h, int rows, int cols) {
   auto* e = static_cast<xb::Estimator*>(h);
-  e->rows = rows; e->cols = cols;
-  e->mask_stride = (cols + 63) / 64;
-  e->mask.assign((size_t)rows * e->mask_stride, 0);
+  e->tracker_set_geometry(rows, cols, true);
   e->reset_mask();
 }
 void hh_mask_reset(void* h) { static_cast<xb::Estimator*>(h)->reset_mask(); }
@@ -264,5 +263,58 @@ void hh_mask_dump(void* h, unsigned char* out) {
   auto* e = static_cast<xb::Estimator*>(h);
   for (int y = 0; y < e->rows; ++y)
     for (int x = 0; x < e->cols; ++x) out[(size_t)y * e->cols + x] = e->mask_bit(x, y) ? 255 : 0;
+}
+
+// ---- image tracker (tracker_host.cpp.inc) with the device phases supplied by the caller; keypoints packed as launch_fast_detect writes them
+static std::vector<std::array<int, 3>> matches_of(const int* m3, int nm) {
+  std::vector<std::array<int, 3>> m((size_t)nm);
+  for (int i = 0; i < nm; ++i) m[i] = {m3[3 * i], m3[3 * i + 1], m3[3 * i + 2]};
+  return m;
+}
+void hh_tracker_geometry(void* h, int rows, int cols) { static_cast<xb::Estimator*>(h)->tracker_set_geometry(rows, cols, true); }
+int hh_tracker_lk_begin(void* h, float* p0, float* p1, int max_pts) { return static_cast<xb::Estimator*>(h)->tracker_lk_begin(p0, p1, max_pts); }
+int hh_tracker_lk_accept(void* h, const float* p0, const float* p1, unsigned char* lkst, const unsigned char* desc, const unsigned char* valid) {
+  return static_cast<xb::Estimator*>(h)->tracker_lk_accept(p0, p1, lkst, desc, valid);
+}
+int hh_tracker_detect_budget(void* h) { return static_cast<xb::Estimator*>(h)->detect_budget; }
+void hh_tracker_detect_select(void* h, const unsigned* kps, int n) { static_cast<xb::Estimator*>(h)->tracker_detect_select(kps, n); }
+int hh_tracker_order_keypoints(void* h, const unsigned* kps, int n, int use_mask, float* kpxy) {
+  return static_cast<xb::Estimator*>(h)->tracker_order_keypoints(kps, n, use_mask != 0, kpxy);
+}
+// descriptors of the query features (32 bytes each); returns their count
+int hh_tracker_queries(void* h, unsigned char* out, int max_n) {
+  auto* e = static_cast<xb::Estimator*>(h);
+  for (size_t i = 0; i < e->query_feats.size() && (int)i < max_n; ++i) memcpy(out + 32 * i, e->query_feats[i]->descriptor, 32);
+  return (int)e->query_feats.size();
+}
+void hh_tracker_detect_select_desc(void* h, const unsigned char* desc, const int* m3, int nm) {
+  static_cast<xb::Estimator*>(h)->tracker_detect_select_desc(desc, matches_of(m3, nm));
+}
+void hh_tracker_lk_finish(void* h) { static_cast<xb::Estimator*>(h)->tracker_lk_finish(); }
+int hh_tracker_match_begin(void* h, const unsigned* kps, int n, float* kpxy) { return static_cast<xb::Estimator*>(h)->tracker_match_begin(kps, n, kpxy); }
+void hh_tracker_match_finish(void* h, const unsigned char* desc, const int* m3, int nm) {
+  static_cast<xb::Estimator*>(h)->tracker_match_finish(desc, matches_of(m3, nm));
+}
+void hh_tracker_only_finish(void* h) { static_cast<xb::Estimator*>(h)->tracker_only_finish(); }
+// per track: id, TrackStatus, last pixel (x, y); returns the track count
+int hh_tracks(void* h, int* ids, int* status, double* xy, int max_n) {
+  auto* e = static_cast<xb::Estimator*>(h);
+  int n = 0;
+  for (xb::Feature* f : e->tracks) {
+    if (n < max_n) { ids[n] = f->id; status[n] = (int)f->tstatus; xy[2 * n] = f->xp()[0]; xy[2 * n + 1] = f->xp()[1]; }
+    ++n;
+  }
+  return n;
+}
+// the descriptor of every track (32 bytes each); returns the track count
+int hh_track_descriptors(void* h, unsigned char* out, int max_n) {
+  auto* e = static_cast<xb::Estimator*>(h);
+  for (size_t i = 0; i < e->tracks.size() && (int)i < max_n; ++i) memcpy(out + 32 * i, e->tracks[i]->descriptor, 32);
+  return (int)e->tracks.size();
+}
+// num_failed_to_track, num_outliers_rejected, num_new_detections
+void hh_tracker_counts(void* h, int* out3) {
+  auto* e = static_cast<xb::Estimator*>(h);
+  out3[0] = e->num_failed_to_track; out3[1] = e->num_outliers_rejected; out3[2] = e->num_new_detections;
 }
 }

@@ -1,6 +1,7 @@
 """The product's host state machine (C++, compiled by g++ into tests/cpp/host_harness.cpp) run through WHOLE point-cloud
 sequences on the CPU, with every device phase (depth sub-filter, Mahalanobis distances, EKF update) replaced by the values the numpy
-oracle computed for the same frame.  Each frame the host's decisions — track list, feature/group slots, in-state and gauge sets, the
+oracle computed for the same frame; the image tracker's host decisions likewise through whole tracker-only image sequences, with the C
+oracle (oracle/tracker_oracle.c) in place of the LK, FAST, BRIEF and matcher kernels.  Each frame the host's decisions — track list, feature/group slots, in-state and gauge sets, the
 features that enter the update, the absorbed pose — must equal the oracle's, and the oracle itself is pinned on the reference's own
 estimator (tests/test_reference_pin.py).  This covers the selection / gating / management logic incl. the libstdc++-defined orders
 (std::unordered_map iteration, unstable std::sort, heap ties) without a GPU; the kernels are covered by the GPU parity tests."""
@@ -14,7 +15,8 @@ import numpy as np
 import pytest
 
 from oracle import estimator_oracle as EO
-from xivo_b200 import sim
+from oracle import tracker_oracle as T
+from xivo_b200 import sim, synth
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 CFG = os.path.join(ROOT, "xivo_b200", "cfg")
@@ -356,3 +358,188 @@ def check_read_back_against_the_reference(hh, h, est, G, F, duration, seed, sim_
     jd = (C.c_int * 512)()
     nj = hh.hh_just_dropped(h, jd, 512)
     assert sorted(jd[:nj]) == sorted(ref["acc.just_dropped"].tolist())
+
+
+# ---- the image tracker (csrc/tracker_host.cpp.inc) against the oracle's Tracker, with the C oracle in place of the kernels ----
+def _tracker_cfg(nmin=60, nmax=80, **tracker):  # as tests/test_gpu_widen_5_descriptors.py: 240 x 320 frames
+    cfg = sim.load_cfg(os.path.join(CFG, "vio_640x480.json"))
+    cfg["camera_cfg"].update(rows=240, cols=320, fx=137.5, fy=137.5, cx=160, cy=120)
+    cfg["message_buffer_size"] = 0
+    cfg["tracker_cfg"].update(num_features_min=nmin, num_features_max=nmax)
+    for k, v in tracker.items():  # (a block given here replaces only the keys it names)
+        cfg["tracker_cfg"][k] = {**cfg["tracker_cfg"].get(k, {}), **v} if isinstance(v, dict) else v
+    return cfg
+
+
+def _frames(seed, n, step=(2, 1), bgr=False, mover=False, jumps=None):
+    pad = 96 if jumps else 64
+    canvas = synth.texture_canvas(240, 320, seed=seed, pad=pad)
+    pos = np.cumsum([(0, 0)] + [(jumps or {}).get(k, step) for k in range(1, n)], axis=0)  # jumps: frame -> its shift from the previous frame
+    out = [synth.frame_from_canvas(canvas, 240, 320, (int(pos[k][0]), int(pos[k][1])), noise_seed=10 * seed + k, pad=pad) for k in range(n)]
+    if mover:  # a block moving against the background: its tracks are the homography's outliers
+        for k, f in enumerate(out):
+            f[60:180, 90:250] = synth.frame_from_canvas(canvas, 240, 320, (-step[0] * k, step[1] * k), noise_seed=10 * seed + k, pad=64)[60:180, 90:250]
+    return [synth.to_bgr(f, distinct=True) for f in out] if bgr else out
+
+
+def _orf(method):
+    return {"method": method, "RANSAC_reproj_thresh": 3.0, "RANSAC_max_iters": 2000, "confidence": 0.995}
+
+
+_DESC = dict(extract_descriptor=True, match_dropped_tracks=True)
+# two sudden camera jumps that LK with few pyramid levels cannot follow: it converges to wrong places, where the descriptor check or the
+# mask drops the tracks while the true keypoints are in view, so the rescue matches them
+_JUMPS = dict(seed=7, n=12, jumps={4: (28, 12), 8: (-24, 10)})
+TRACKER_CASES = {
+    # low FAST threshold and a small mask: thousands of keypoints in a narrow score band (ties resolved by (y, x)); on the second of two
+    # blank frames every track is lost and nothing is detected, the next frame finds an empty list and the one after re-initialises
+    "lk_ties_blank": (_tracker_cfg(300, 400, mask_size=5, margin=4, FAST={"threshold": 5, "nonmaxSuppression": True}), dict(seed=3, n=10, blank=4)),
+    "lk_bgr": (_tracker_cfg(75, 100, FAST={"threshold": 20, "nonmaxSuppression": True}), dict(seed=4, n=8, bgr=True)),
+    "lk_outliers_lmeds": (_tracker_cfg(do_outlier_rejection=True, outlier_rejection=_orf("LMEDS")), dict(seed=5, n=10, step=(3, 2), mover=True)),
+    "lk_outliers_ransac": (_tracker_cfg(do_outlier_rejection=True, outlier_rejection=_orf("RANSAC")), dict(seed=6, n=10, step=(3, 2), mover=True)),
+    # (num_features_min = max: a detection every frame with a small budget, which a rescue can use up)
+    "rescue_like_tumvi_cam0": (_tracker_cfg(80, 80, **_DESC, differential=False, descriptor_distance_thresh=-1, KLT={"max_level": 2}), dict(_JUMPS, seed=12)),
+    "distance_check_differential": (_tracker_cfg(**_DESC, differential=True, descriptor_distance_thresh=70, KLT={"max_level": 0}), _JUMPS),
+    "rescue_with_outlier_rejection": (_tracker_cfg(**_DESC, differential=True, do_outlier_rejection=True, outlier_rejection=_orf("LMEDS"),
+                                                   KLT={"max_level": 1}), dict(_JUMPS, mover=True)),
+    "match": (_tracker_cfg(tracker_type="MATCH", extract_descriptor=True, differential=True, descriptor_distance_thresh=-1), dict(seed=10, n=12, step=(3, 2))),
+    "match_outliers_lmeds": (_tracker_cfg(tracker_type="MATCH", extract_descriptor=True, differential=True, descriptor_distance_thresh=-1, do_outlier_rejection=True,
+                                          outlier_rejection=_orf("LMEDS")), dict(seed=11, n=10, step=(3, 2), mover=True)),
+}
+
+
+def _pack(xy, sc):  # launch_fast_detect's keypoint format: y << 20 | x << 8 | score
+    assert len(sc) == 0 or sc.max() <= 255
+    return np.ascontiguousarray((xy[:, 1].astype(np.uint32) << 20) | (xy[:, 0].astype(np.uint32) << 8) | sc.astype(np.uint32))
+
+
+def _ptr(a):
+    return a.ctypes.data if a is not None else None
+
+
+@pytest.mark.parametrize("case", list(TRACKER_CASES))
+def test_image_tracker_follows_the_oracle_frame_by_frame(hh, case):
+    cfg, fr = TRACKER_CASES[case]
+    frames = _frames(fr["seed"], fr["n"], fr.get("step", (2, 1)), fr.get("bgr", False), fr.get("mover", False), fr.get("jumps"))
+    if "blank" in fr:
+        frames[fr["blank"]:fr["blank"]] = [np.full((240, 320), 128, np.uint8)] * 2
+    for n, t in (("hh_tracker_lk_begin", [C.c_void_p] * 3 + [C.c_int]), ("hh_tracker_lk_accept", [C.c_void_p] * 6),
+                 ("hh_tracker_detect_select", [C.c_void_p] * 2 + [C.c_int]), ("hh_tracker_order_keypoints", [C.c_void_p] * 2 + [C.c_int] * 2 + [C.c_void_p]),
+                 ("hh_tracker_queries", [C.c_void_p] * 2 + [C.c_int]), ("hh_tracker_detect_select_desc", [C.c_void_p] * 3 + [C.c_int]),
+                 ("hh_tracker_match_begin", [C.c_void_p] * 2 + [C.c_int, C.c_void_p]), ("hh_tracker_match_finish", [C.c_void_p] * 3 + [C.c_int]),
+                 ("hh_tracks", [C.c_void_p] * 4 + [C.c_int]), ("hh_track_descriptors", [C.c_void_p] * 2 + [C.c_int]), ("hh_tracker_counts", [C.c_void_p] * 2), ("hh_tracker_geometry", [C.c_void_p, C.c_int, C.c_int]),
+                 ("hh_visual_begin", [C.c_void_p, C.c_ulonglong, C.c_int])):
+        getattr(hh, n).argtypes = t
+    for n in ("hh_tracker_detect_budget", "hh_tracker_lk_finish", "hh_tracker_only_finish"):
+        getattr(hh, n).argtypes = [C.c_void_p]
+    est = EO.EstimatorOracle(cfg, G=4, F=14, tracker_only=True)
+    h = hh.hh_create(json.dumps(cfg).encode(), 4, 14, 1)
+    assert h, hh.hh_error()
+    hh.hh_tracker_geometry(h, 240, 320)
+    max_pts = est.t_max + 8
+    p0, p1 = np.zeros((max_pts, 2), np.float32), np.zeros((max_pts, 2), np.float32)
+    qd = np.zeros((max_pts, 32), np.uint8)
+    ids, st, xy, tdesc = np.zeros(4096, np.int32), np.zeros(4096, np.int32), np.zeros((4096, 2)), np.zeros((4096, 32), np.uint8)
+    cnt = np.zeros(3, np.int32)
+
+    def detect(img):
+        kxy, sc, _ = T.fast_detect(img, est.fast_thr, est.fast_nms)
+        return _pack(kxy, sc)
+
+    def describe_and_match(img, nk, kpxy):
+        D = np.ascontiguousarray(T.brief(img, kpxy[:nk])[0]) if nk else np.zeros((1, 32), np.uint8)
+        nq = hh.hh_tracker_queries(h, _ptr(qd), max_pts)
+        m = np.ascontiguousarray(T.bf_match_crosscheck(qd[:nq], D[:nk]) if nq and nk else np.zeros((0, 3)), np.int32).reshape(-1, 3)
+        return D, m
+
+    # DetectLK's outcome before UpdateLK marks the newly dropped tracks DROPPED again (what a rescue did to a track is visible only here):
+    # the oracle's track list right after detect_lk
+    snap, n_rescued, n_dist_drops, n_candidates = [], 0, 0, 0
+    detect0 = est.detect_lk
+
+    def detect_lk(img, num_to_add, newly_dropped=(), check_homography=False):
+        nonlocal n_rescued
+        seen = {f.id: len(f.track) for f in newly_dropped}
+        detect0(img, num_to_add, newly_dropped, check_homography)
+        # the product marks a newly dropped track DROPPED before DetectLK, the oracle after it; a rescued one is TRACKED in both
+        rescued = {f.id for f in newly_dropped if len(f.track) > seen[f.id]}
+        n_rescued += len(rescued)
+        status = lambda f: int(EO.TRACKED if f.id in rescued else EO.DROPPED) if f.id in seen else int(f.tstatus)
+        snap.append([(f.id, status(f), float(f.xp()[0]), float(f.xp()[1]), bytes(np.asarray(f.descriptor, np.uint8).tobytes()) if est.extract_descriptor else b"")
+                     for f in est.tracks])
+
+    est.detect_lk = detect_lk
+
+    def snapshot():
+        n = hh.hh_tracks(h, _ptr(ids), _ptr(st), _ptr(xy), len(ids))
+        hh.hh_track_descriptors(h, _ptr(tdesc), len(tdesc))
+        return [(int(ids[i]), int(st[i]), float(xy[i, 0]), float(xy[i, 1]), tdesc[i].tobytes() if est.extract_descriptor else b"") for i in range(n)]
+
+    prev, tracks_seen, rejected = None, [], []
+    for k, img in enumerate(frames):
+        ts = (k + 1) * 40_000_000
+        vc = est.vision_counter
+        est.VisualMeasTrackerOnly(ts, img)
+        assert est.vision_counter == vc + 1
+        assert hh.hh_visual_begin(h, ts, 2) == 1
+        if est.tracker_type == "MATCH":
+            kps = detect(img)
+            kpxy = np.zeros((max(1, len(kps)), 2), np.float32)
+            nk = hh.hh_tracker_match_begin(h, _ptr(kps), len(kps), _ptr(kpxy))
+            D, m = describe_and_match(img, nk, kpxy)
+            hh.hh_tracker_match_finish(h, _ptr(D), _ptr(m), len(m))
+        else:
+            ntr = hh.hh_tracks(h, _ptr(ids), _ptr(st), _ptr(xy), len(ids))
+            kind = hh.hh_tracker_lk_begin(h, _ptr(p0), _ptr(p1), max_pts)
+            assert kind in (1, 2, 3), f"frame {k}: kind {kind}"
+            if kind == 2:  # the LK kernel on the points the host staged
+                r1, lkst, _ = T.lk_track(prev, img, p0[:ntr], p1[:ntr], **est.klt)
+                r1, lkst = np.ascontiguousarray(r1, np.float32), np.ascontiguousarray(lkst, np.uint8)
+                d = v = None
+                if est.extract_descriptor:
+                    d, v = T.brief(img, r1)
+                    d, v = np.ascontiguousarray(d), np.ascontiguousarray(v, np.uint8)
+                lkst0 = lkst.copy()
+                hh.hh_tracker_lk_accept(h, _ptr(p0), _ptr(r1), _ptr(lkst), _ptr(d), _ptr(v))
+                n_dist_drops += int((lkst0 > lkst).sum())  # tracks the descriptor-distance check dropped
+            if kind != 3:
+                if hh.hh_tracker_detect_budget(h) > 0:
+                    kps = detect(img)
+                    if not est.extract_descriptor:
+                        hh.hh_tracker_detect_select(h, _ptr(kps), len(kps))
+                    else:
+                        kpxy = np.zeros((max(1, len(kps)), 2), np.float32)
+                        nk = hh.hh_tracker_order_keypoints(h, _ptr(kps), len(kps), 1, _ptr(kpxy))
+                        D, m = describe_and_match(img, nk, kpxy)
+                        hh.hh_tracker_detect_select_desc(h, _ptr(D), _ptr(m), len(m))
+                        n_candidates += len(m)
+                    assert snapshot() == snap.pop(0), f"frame {k}: track list after DetectLK"
+                prev = img
+            hh.hh_tracker_lk_finish(h)
+        hh.hh_tracker_only_finish(h)
+        assert hh.hh_sticky_error(h) == 0, hh.hh_error_msg(h)
+        assert not snap, f"frame {k}: the oracle detected, the product did not"
+        n = hh.hh_tracks(h, _ptr(ids), _ptr(st), _ptr(xy), len(ids))
+        assert ids[:n].tolist() == [f.id for f in est.tracks], f"frame {k}: track ids / order"
+        assert st[:n].tolist() == [int(f.tstatus) for f in est.tracks], f"frame {k}: TrackStatus"
+        assert np.array_equal(xy[:n], np.array([f.xp() for f in est.tracks]).reshape(-1, 2)), f"frame {k}: positions"
+        hh.hh_tracker_counts(h, _ptr(cnt))
+        assert (cnt[0], cnt[1]) == (est.num_failed_to_track, est.num_outliers_rejected), f"frame {k}: failed / outlier counts"
+        if est.tracker_type == "MATCH":
+            assert cnt[2] == est.num_new_detections, f"frame {k}: new detections"
+        tracks_seen.append(n)
+        rejected.append(int(cnt[1]))
+    hh.hh_destroy(h)
+    print(case, "frames", len(frames), "tracks per frame", tracks_seen, "outliers rejected", rejected, "rescued", n_rescued, "of", n_candidates, "candidates", "distance-check drops", n_dist_drops)
+    assert max(tracks_seen) >= 0.9 * est.t_max
+    if "blank" in fr:
+        b = fr["blank"]
+        assert tracks_seen[b + 1] == tracks_seen[b + 2] == 0 and tracks_seen[b + 3] == est.t_max, "the blank frames force a re-initialisation"
+    if est.do_outlier_rejection:
+        assert sum(rejected) >= 50, "the homography rejection must reject tracks"
+    if est.match_dropped and not est.do_outlier_rejection:
+        assert n_rescued >= 5, "the rescue of newly dropped tracks must be exercised"
+    if est.match_dropped and est.do_outlier_rejection:  # CheckHomography compares the creation keypoint: under camera motion it rejects them all
+        assert n_candidates >= 5, "cross-checked matches must reach the homography check of the rescue"
+    if est.desc_thresh > 0 and est.tracker_type == "LK":
+        assert n_dist_drops >= 5, "the descriptor-distance check must drop tracks"

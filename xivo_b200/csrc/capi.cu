@@ -141,9 +141,9 @@ int xivo_fast_detect(xivo_ctx* ctx, const uint8_t* img, int rows, int cols, int 
   std::sort(kp.begin(), kp.end());  // packed (y, x, score): ascending == raster order
   *n_kp = cnt;
   for (int i = 0; i < std::min(got, max_kp); ++i) {
-    kp_xy[2 * i] = (kp[i] >> 8) & 0xfff;
-    kp_xy[2 * i + 1] = kp[i] >> 20;
-    kp_score[i] = kp[i] & 0xff;
+    kp_xy[2 * i] = xb::kp_x(kp[i]);
+    kp_xy[2 * i + 1] = xb::kp_y(kp[i]);
+    kp_score[i] = xb::kp_score(kp[i]);
   }
   return XIVO_OK;
 }

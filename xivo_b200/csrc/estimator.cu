@@ -1,5 +1,5 @@
 // Estimator-level C ABI (include/xivo_b200_estimator.h): a Batch of independent estimators that
-// advance in lock-step.  The host state machines (estimator_host.cpp.inc) decide; every numeric hot
+// advance in lock-step.  The host state machines (estimator_host.cpp.inc, tracker_host.cpp.inc) decide; every numeric hot
 // loop runs in the CUDA kernels of tracker_kernels.cu / ekf_kernels.cu, batched over sequences.
 
 #include <algorithm>
@@ -8,6 +8,7 @@
 #include <cstring>
 #include <deque>
 #include <mutex>
+#include <optional>
 #include <stdexcept>
 
 #include "../../include/xivo_b200_estimator.h"
@@ -36,6 +37,7 @@ struct HostScope {
 }  // namespace xb
 
 #include "estimator_host.cpp.inc"
+#include "tracker_host.cpp.inc"
 
 namespace xb {
 extern std::atomic<unsigned long long> g_launches;
@@ -269,8 +271,6 @@ class Batch {
   Mirror<int> nkps, nq;                 // B
   Mirror<uint8_t> descK, validK, qdesc; // B x max_kp x 32 / B x max_kp / B x max_pts x 32 (queries: descriptors of dropped / existing tracks)
   Mirror<int> bestT_idx, bestT_dist, bestQ_idx, bestQ_dist;  // nearest keypoint of every query; nearest query of every keypoint
-  std::vector<std::vector<unsigned>> sorted_kp;   // per sequence: packed keypoints (y << 20 | x << 8 | score) in selection order
-  std::vector<std::vector<Feature*>> query_feats; // per sequence: the features behind the query descriptors
   // every table of the tracker phase lives in ONE blob: [inputs | pts1 (in/out) | outputs], so the phase costs one H2D and one D2H call
   Mirror<unsigned char> tt;
   size_t tt_up_bytes = 0, tt_down_off = 0, tt_down_bytes = 0;
@@ -406,14 +406,11 @@ class Batch {
     e->compact_records = true;
     e->sim_initialize_depths = sim_depths;
     if (img_ready) {  // what ensure_images gives every estimator at the first image
-      e->rows = rows; e->cols = cols;
-      e->mask_stride = (cols + 63) / 64;
-      if (!dev_decide) e->mask.assign((size_t)rows * e->mask_stride, 0);
+      e->tracker_set_geometry(rows, cols, !dev_decide);
       prev_slot[seq] = 0;
     }
-    est[seq] = std::move(e);  // the old estimator's heap, pending propagation records and edits go with it
+    est[seq] = std::move(e);  // the old estimator's heap, pending propagation records, edits and tracker state go with it
     table_order[seq].clear();
-    if (desc_on) { sorted_kp[seq].clear(); query_feats[seq].clear(); }
     if (!pref.empty()) {  // pending prefetches are dropped as take_slots drops them: their slots are handed out again
       for (int s = 0; s < B; ++s) ring_next[s] = pref.front().slot[s];
       pref.clear();
@@ -745,8 +742,6 @@ class Batch {
       const size_t npt = (size_t)B * max_pts, nk = (size_t)B * max_kp;
       ok = descT.alloc(npt * 32) && validT.alloc(npt) && kpxy.alloc(nk * 2) && nkps.alloc(B) && nq.alloc(B) && descK.alloc(nk * 32) && validK.alloc(nk) &&
            qdesc.alloc(npt * 32) && bestT_idx.alloc(npt) && bestT_dist.alloc(npt) && bestQ_idx.alloc(nk) && bestQ_dist.alloc(nk);
-      sorted_kp.resize(B);
-      query_feats.resize(B);
     }
     if (ok) {
       ingest_ptr.adopt(blobG.h, blobG.d, B);
@@ -793,76 +788,84 @@ class Batch {
     ring_ev.resize(ring_n);
     for (auto& e : ring_ev) cudaEventCreateWithFlags(&e, cudaEventDisableTiming);
     prev_slot.assign(B, 0);
-    for (auto& e : est) {
-      e->rows = rows; e->cols = cols;
-      e->mask_stride = (cols + 63) / 64;
-      if (!dev_decide) e->mask.assign((size_t)rows * e->mask_stride, 0);  // the host bitmap exists only on the host-decision path
-    }
+    for (auto& e : est) e->tracker_set_geometry(rows, cols, !dev_decide);
     img_ready = true;
     return 0;
   }
 
-  // Tracker::DetectLK's selection (tracker.cpp:224-229, :295-328) from the packed keypoints of one sequence.
-  void detect_select(Estimator& e, const unsigned* kps, int n, int num_to_add) {
-    // runByPixelsMask, then order (score desc, y asc, x asc): counting sort by score into one reusable
-    // array, each score bucket sorted lazily (the greedy pick usually stops in the first few buckets).
-    static thread_local std::vector<unsigned> sorted;
-    int cnt[257] = {0};
-    for (int i = 0; i < n; ++i) {
-      const unsigned k = kps[i];
-      if (e.mask_bit((k >> 8) & 0xfff, k >> 20)) cnt[(k & 0xff) + 1]++;
+  // The frame of every sequence in `act` (ring slot slots[i]) goes into the free half of the sequence's pyramid buffer: the tracker stream
+  // waits for the slots' uploads; off_cur / off_prev / frame_ptr (and the TMA image indices) of the sequences, ~0 / 0 for the others.
+  int begin_frame(const std::vector<int>& act, const std::vector<int>& slots) {
+    const size_t ib = (size_t)rows * cols * cn;
+    for (int b = 0; b < B; ++b) { off_cur.h[b] = ~0ull; off_prev.h[b] = 0; npts.h[b] = 0; }
+    std::vector<char> seen(ring_n, 0);
+    for (int k : slots)
+      if (!seen[k]) { seen[k] = 1; XB_CUDA(cudaStreamWaitEvent(st1, ring_ev[k], 0)); }
+    for (size_t i = 0; i < act.size(); ++i) {
+      const int b = act[i];
+      const int cur = 1 - prev_slot[b];
+      off_cur.h[b] = ((size_t)b * 2 + cur) * pd.total;
+      off_prev.h[b] = ((size_t)b * 2 + prev_slot[b]) * pd.total;
+      frame_ptr.h[b] = dRing + ((size_t)b * ring_n + slots[i]) * ib;  // consumed by the first pyrDown pass
+      if (tma_pyr) { ring_img.h[b] = b * ring_n + slots[i]; pyr_img.h[b] = b * 2 + cur; }
     }
-    for (int s = 0; s < 256; ++s) cnt[s + 1] += cnt[s];  // cnt[s] = start of bucket s
-    sorted.resize(cnt[256]);
-    int cursor[256];
-    for (int s = 0; s < 256; ++s) cursor[s] = cnt[s];
-    for (int i = 0; i < n; ++i) {
-      const unsigned k = kps[i];
-      if (e.mask_bit((k >> 8) & 0xfff, k >> 20)) sorted[cursor[k & 0xff]++] = k;
-    }
-    for (int s = 255; s >= 0; --s) {
-      if (cnt[s + 1] == cnt[s]) continue;
-      std::sort(sorted.begin() + cnt[s], sorted.begin() + cnt[s + 1]);  // packed (y, x, score): (y, x) ascending within a score
-      for (int i = cnt[s]; i < cnt[s + 1]; ++i) {
-        const unsigned k = sorted[i];
-        const double x = (k >> 8) & 0xfff, y = k >> 20;
-        if (e.mask_valid(x, y)) {
-          Feature* f = e.create_feature(x, y);
-          if (!f) return;
-          f->response = (float)s;
-          e.tracks.push_back(f);
-          e.num_new_detections++;
-          e.mask_out(x, y);
-          --num_to_add;
-        }
-        if (num_to_add <= 0 || s < 5) return;
+    return 0;
+  }
+  // The pyramid passes of the frames begun by begin_frame: every level (LK), or level 0 only (MATCH: the image FAST and BRIEF read).
+  int build_pyramids(bool all_levels) {
+    if (tma_pyr) {
+      std::optional<ProfScope> ps;
+      if (all_levels) ps.emplace("pyrdown", st1);
+      if (int rc = launch_pyrdown_tma(st1, tm_ring, ring_img.d, dPyr, 0, off_cur.d, pd, 0, 1, B)) return rc;
+      for (int l = 1; all_levels && l + 1 < pd.n_levels; ++l) {
+        if (tm_lvl_ok[l]) { if (int rc = launch_pyrdown_tma(st1, tm_lvl[l], pyr_img.d, dPyr, 0, off_cur.d, pd, l, 0, B)) return rc; }
+        else if (int rc = launch_pyrdown_level(st1, dPyr, 0, off_cur.d, pd, B, nullptr, l)) return rc;
       }
+    } else if (int rc = all_levels ? launch_build_pyramid(st1, dPyr, 0, off_cur.d, pd, B, frame_ptr.d) : launch_pyrdown_level(st1, dPyr, 0, off_cur.d, pd, B, frame_ptr.d, 0))
+      return rc;
+    g_launches += all_levels ? std::max(1, pd.n_levels - 1) : 1;
+    return 0;
+  }
+  // FAST on the level-0 images that sel selects (device pyramid offsets, ~0 = skip), then the keypoint counts and the keypoints of `seqs`.
+  int detect_and_fetch(const std::vector<int>& seqs, const unsigned long long* sel) {
+    cudaStream_t st = st1;
+    const TrackerCfg& tc = est[0]->tc;
+    if (int rc = launch_fast_detect(st, dPyr, 0, sel, rows, cols, cn, tc.fast_threshold, tc.fast_nonmax, kp.d, max_kp, kpcount.d, B, nullptr,
+                                    tma_fast ? &tm_fast : nullptr, pd.total))
+      return rc;
+    g_launches += 1;
+    XB_CUDA(kpcount.down(st));
+    { HostScope hw("wait_fastcount"); if (int rc = wait(st)) return rc; }
+    for (int b : seqs) {
+      const int n = std::min(kpcount.h[b], max_kp);
+      if (n) { Prof::get().d2h += sizeof(unsigned) * n; XB_CUDA(cudaMemcpyAsync(kp.h + (size_t)b * max_kp, kp.d + (size_t)b * max_kp, sizeof(unsigned) * n, cudaMemcpyDeviceToHost, st)); }
     }
+    HostScope hw("wait_fastkp");
+    return wait(st);
+  }
+  // LK of the staged points (pts0 -> pts1) from the previous to the current pyramid of every sequence with npts > 0
+  int track_lk(const std::vector<int>& lk_list) {
+    const TrackerCfg& tc = est[0]->tc;
+    if (int rc = launch_lk_track(st1, dPyr, dPyr, 0, off_prev.d, off_cur.d, pd, pts0.d, pts1.d, lkst.d, lkerr.d, npts.d, max_pts, B, tc.win_size, tc.max_iter,
+                                 tc.eps, 1, 1e-4))
+      return rc;
+    g_launches += 1;
+    double np_ = 0;
+    for (int b : lk_list) np_ += npts.h[b];
+    Prof::get().add_work("lk_track", np_ * pd.n_levels * (17.0 * 17.0 + 25.0 * 25.0) * cn);  // §8d: L (17^2+25^2) c bytes / feature
+    return 0;
+  }
+  void swap_pyramids(const std::vector<int>& act) {
+    for (int b : act)
+      if (off_cur.h[b] != ~0ull) prev_slot[b] = 1 - prev_slot[b];  // std::swap(pyramid, pyramid_)
+  }
+  // cross-checked matches of sequence b from the nearest-neighbour tables of describe_and_match
+  void matches_of(int b, std::vector<std::array<int, 3>>* m) const {
+    cross_checked(nq.h[b], bestT_idx.h + (size_t)b * max_pts, bestT_dist.h + (size_t)b * max_pts, bestQ_idx.h + (size_t)b * max_kp, m);
   }
 
-  // Detected keypoints of one sequence in the order DetectLK / UpdateMatch walks them: [mask filter (detect(img, kps, mask_))] -> sort by
-  // response (total order (score desc, y, x): the reference's std::sort is unstable) -> the descriptor extractor drops the 28-pixel border band.
-  void order_keypoints(int b, const unsigned* kps, int n, bool use_mask) {
-    Estimator& e = *est[b];
-    std::vector<unsigned>& v = sorted_kp[b];
-    v.clear();
-    for (int i = 0; i < n; ++i) {
-      const unsigned k = kps[i];
-      const int x = (k >> 8) & 0xfff, y = k >> 20;
-      if (use_mask && !e.mask_bit(x, y)) continue;
-      if (x < 28 || x >= cols - 28 || y < 28 || y >= rows - 28) continue;  // KeyPointsFilter::runByImageBorder(.., 48 / 2 + 9 / 2)
-      v.push_back(k);
-    }
-    std::sort(v.begin(), v.end(), [](unsigned a, unsigned c) {
-      const unsigned sa = a & 0xff, sc = c & 0xff;
-      return sa != sc ? sa > sc : (a >> 8) < (c >> 8);  // (y, x) ascending within a score
-    });
-    float* xy = kpxy.h + (size_t)b * max_kp * 2;
-    for (size_t i = 0; i < v.size(); ++i) { xy[2 * i] = (float)((v[i] >> 8) & 0xfff); xy[2 * i + 1] = (float)(v[i] >> 20); }
-    nkps.h[b] = (int)v.size();
-  }
   // BRIEF at the ordered keypoints of `seqs` (level-0 image of the current pyramid: sel_off) and, where a sequence has query descriptors
-  // (query_feats), the two nearest-neighbour tables of the cross-checked matcher.  One wait.
+  // (Estimator::query_feats), the two nearest-neighbour tables of the cross-checked matcher.  One wait.
   int describe_and_match(const std::vector<int>& seqs, const unsigned long long* sel_off_dev) {
     cudaStream_t st = st1;
     bool any_q = false;
@@ -870,10 +873,10 @@ class Batch {
     for (int b : seqs) {
       const int n = nkps.h[b];
       if (n) XB_CUDA(cudaMemcpyAsync(kpxy.d + (size_t)b * max_kp * 2, kpxy.h + (size_t)b * max_kp * 2, sizeof(float) * 2 * n, cudaMemcpyHostToDevice, st));
-      const int q = (int)query_feats[b].size();
-      if (q > max_pts) return fail(XIVO_ERR_STATE, "descriptor matcher: more query features than max_pts");
-      nq.h[b] = n ? q : 0;
-      for (int j = 0; j < nq.h[b]; ++j) memcpy(qdesc.h + ((size_t)b * max_pts + j) * 32, query_feats[b][j]->descriptor, 32);
+      const std::vector<Feature*>& qf = est[b]->query_feats;
+      if ((int)qf.size() > max_pts) return fail(XIVO_ERR_STATE, "descriptor matcher: more query features than max_pts");
+      nq.h[b] = n ? (int)qf.size() : 0;
+      for (int j = 0; j < nq.h[b]; ++j) memcpy(qdesc.h + ((size_t)b * max_pts + j) * 32, qf[j]->descriptor, 32);
       if (nq.h[b]) {
         any_q = true;
         XB_CUDA(cudaMemcpyAsync(qdesc.d + (size_t)b * max_pts * 32, qdesc.h + (size_t)b * max_pts * 32, (size_t)32 * nq.h[b], cudaMemcpyHostToDevice, st));
@@ -900,69 +903,12 @@ class Batch {
     HostScope hw("wait_describe");
     return wait(st);
   }
-  // cross-checked matches of sequence b as (query, keypoint, distance), in query order (cv::BFMatcher::knnMatch with compactResult)
-  void cross_checked(int b, std::vector<std::array<int, 3>>* out) const {
-    out->clear();
-    for (int q = 0; q < nq.h[b]; ++q) {
-      const int t = bestT_idx.h[(size_t)b * max_pts + q];
-      if (t >= 0 && bestQ_idx.h[(size_t)b * max_kp + t] == q) out->push_back({q, t, bestT_dist.h[(size_t)b * max_pts + q]});
-    }
-  }
-  // Tracker::DetectLK with descriptors (tracker.cpp:231-327): rescue matching of the newly dropped tracks, then the greedy pick.
-  void detect_select_desc(int b, int num_to_add, bool check_homography) {
-    Estimator& e = *est[b];
-    const std::vector<unsigned>& v = sorted_kp[b];
-    const uint8_t* D = descK.h + (size_t)b * max_kp * 32;
-    std::vector<int> match_of(v.size(), -1);  // keypoint -> index into query_feats[b] (the newly dropped tracks)
-    if (e.tc.match_dropped_tracks && nq.h[b] && !v.empty()) {
-      std::vector<std::array<int, 3>> m;
-      cross_checked(b, &m);
-      for (const auto& d : m) {
-        Feature* f = query_feats[b][d[0]];
-        const double x = (v[d[1]] >> 8) & 0xfff, y = v[d[1]] >> 20;
-        const bool ok_desc = e.tc.descriptor_distance_thresh > 0 ? d[2] < e.tc.descriptor_distance_thresh : true;  // CheckDescriptorDistance
-        const double dx = x - f->xp()[0], dy = y - f->xp()[1];
-        const bool ok_disp = std::sqrt(dx * dx + dy * dy) < e.tc.max_pixel_displacement;
-        bool ok_h = true;
-        if (check_homography) {  // CheckHomography (tracker.cpp:818-828) never applies H: |creation keypoint - new keypoint| < reprojection threshold
-          const double hx = (double)f->kp0[0] - x, hy = (double)f->kp0[1] - y;
-          ok_h = std::sqrt(hx * hx + hy * hy) < e.tc.outlier_reproj_thresh;
-        }
-        if (ok_desc && ok_disp && ok_h) match_of[d[1]] = d[0];
-      }
-    }
-    for (size_t i = 0; i < v.size(); ++i) {
-      const unsigned k = v[i];
-      const double x = (k >> 8) & 0xfff, y = k >> 20;
-      if (e.mask_valid(x, y)) {
-        if (e.tc.match_dropped_tracks && match_of[i] >= 0) {
-          Feature* f1 = query_feats[b][match_of[i]];
-          if (e.tc.differential) memcpy(f1->descriptor, D + 32 * i, 32);
-          f1->observe(x, y);
-          f1->tstatus = TrackStatus::TRACKED;  // "potentially rescued": UpdateLK marks every newly dropped track DROPPED right after (tracker.cpp:617-619)
-          e.mask_out(x, y);
-          --num_to_add;
-          continue;  // (skips the budget / response test, like the reference)
-        }
-        Feature* f = e.create_feature(x, y);
-        if (!f) return;
-        f->response = (float)(k & 0xff);
-        memcpy(f->descriptor, D + 32 * i, 32);
-        f->has_descriptor = true;
-        e.tracks.push_back(f);
-        e.num_new_detections++;
-        e.mask_out(x, y);
-        --num_to_add;
-      }
-      if (num_to_add <= 0 || (k & 0xff) < 5) return;
-    }
-  }
 
   // The rest of Tracker::UpdateLK with the decisions on the device: LK -> accept loop (track_accept_kernel) -> FAST for the sequences
   // the accept kernel flagged -> greedy selection (track_select_kernel) -> ONE read-back of [positions | keep flags | picks].  The host
   // then only replays the decisions on its track list (same order, same feature ids as the host path).
-  int tracker_decide_on_device(const std::vector<int>& act, const std::vector<int>& lk_list, const std::vector<int>& det_first,
-                               const std::vector<int>& kind, std::unique_ptr<HostScope>* hs_issue) {
+  int tracker_decide_on_device(const std::vector<int>& act, const std::vector<int>& lk_list, const std::vector<int>& kind,
+                               std::unique_ptr<HostScope>* hs_issue) {
     cudaStream_t st = st1;
     const TrackerCfg& tc = est[0]->tc;
     Estimator& e0 = *est[0];
@@ -972,13 +918,7 @@ class Batch {
                       (double)tc.max_pixel_displacement};
     if (!lk_list.empty()) {
       HostScope hx("x_i_trk_lk");
-      if (int rc = launch_lk_track(st, dPyr, dPyr, 0, off_prev.d, off_cur.d, pd, pts0.d, pts1.d, lkst.d, lkerr.d, npts.d, max_pts, B,
-                                   tc.win_size, tc.max_iter, tc.eps, 1, 1e-4))
-        return rc;
-      g_launches += 1;
-      double np_ = 0;
-      for (int b : lk_list) np_ += npts.h[b];
-      Prof::get().add_work("lk_track", np_ * pd.n_levels * (17.0 * 17.0 + 25.0 * 25.0) * cn);  // §8d: L (17^2+25^2) c bytes / feature
+      if (int rc = track_lk(lk_list)) return rc;
     }
     {
       HostScope hx("x_i_trk_accept");
@@ -1005,109 +945,33 @@ class Batch {
     HostScope hs("tracker_accept");
     pfor(act, [&](int b, int) {
       HostScope hx("x_trk_replay");
-      Estimator& e = *est[b];
-      if (kind[b] == 3) return;
-      if (kind[b] == 2) {
-        int i = 0, num_failed = 0;
-        for (Feature* f : e.tracks) {
-          prefetch_ahead(e.tracks, (size_t)i, 2);
-          const float* p1 = pts1.h + ((size_t)b * max_pts + i) * 2;
-          if (tstat.h[(size_t)b * max_pts + i]) {
-            f->tstatus = TrackStatus::TRACKED;
-            f->observe((double)p1[0], (double)p1[1]);
-          } else {
-            f->tstatus = TrackStatus::DROPPED;
-            ++num_failed;
-          }
-          ++i;
-        }
-        e.num_new_detections = 0;
-        e.num_failed_to_track = num_failed;
-      }
-      if (tneed.h[b] > 0) {
-        const int nn = std::min(tnnew.h[b], max_new);
-        for (int j = 0; j < nn; ++j) {
-          const unsigned k = tnewkp.h[(size_t)b * max_new + j];
-          Feature* f = e.create_feature((double)((k >> 8) & 0xfff), (double)(k >> 20));
-          if (!f) return;
-          f->response = (float)(k & 0xff);
-          e.tracks.push_back(f);
-          e.num_new_detections++;
-        }
-        e.tracker_initialized = true;
-      }
+      est[b]->tracker_replay(kind[b], pts1.h + (size_t)b * max_pts * 2, tstat.h + (size_t)b * max_pts, tneed.h[b], tnewkp.h + (size_t)b * max_new,
+                             std::min(tnnew.h[b], max_new));
     });
-    for (int b : act)
-      if (off_cur.h[b] != ~0ull) prev_slot[b] = 1 - prev_slot[b];  // std::swap(pyramid, pyramid_)
+    swap_pyramids(act);
     return 0;
   }
 
-  // Tracker::UpdateLK (tracker.cpp:463-629) for the sequences in `act` whose message holds ring slot
-  // slots[i].  Descriptor / rescue / homography branches are out of scope (SURVEY.md §8f).
+  // Tracker::UpdateLK (tracker.cpp:463-629) for the sequences in `act` whose message holds ring slot slots[i]; the decisions are the
+  // estimators' (tracker_host.cpp.inc) or, without descriptors and homography rejection, the device's (tracker_decide_on_device).
   int tracker_update_lk(const std::vector<int>& act, const std::vector<int>& slots) {
     cudaStream_t st = st1;
-    const size_t ib = (size_t)rows * cols * cn;
-    std::vector<int> lk_list, det_list;
-    std::vector<char> check_h(B, 0);  // DetectLK's check_homography: the frame's outlier rejection ran
-    if (desc_on)
-      for (int b : act) query_feats[b].clear();
-    std::vector<int> det_budget(B, 0), kind(B, 0);  // kind: 1 = first frame (detect only), 2 = LK, 3 = empty list
-    for (int b = 0; b < B; ++b) { off_cur.h[b] = ~0ull; off_prev.h[b] = 0; npts.h[b] = 0; }
-    std::atomic<int> overflow{0};
+    std::vector<int> lk_list, det_list, kind(B, 0);
     {
       HostScope hs("tracker_prepare");
-      {
-        std::vector<char> seen(ring_n, 0);
-        for (int k : slots)
-          if (!seen[k]) { seen[k] = 1; XB_CUDA(cudaStreamWaitEvent(st, ring_ev[k], 0)); }
-      }
-      for (size_t i = 0; i < act.size(); ++i) {
-        const int b = act[i];
-        const int cur = 1 - prev_slot[b];
-        off_cur.h[b] = ((size_t)b * 2 + cur) * pd.total;
-        off_prev.h[b] = ((size_t)b * 2 + prev_slot[b]) * pd.total;
-        frame_ptr.h[b] = dRing + ((size_t)b * ring_n + slots[i]) * ib;  // consumed by the first pyrDown pass
-        if (tma_pyr) { ring_img.h[b] = b * ring_n + slots[i]; pyr_img.h[b] = b * 2 + cur; }
-      }
+      if (int rc = begin_frame(act, slots)) return rc;
+      std::atomic<int> overflow{0};
       pfor(act, [&](int b, int) {
         HostScope hx("x_trk_prepare");
         Estimator& e = *est[b];
-        if (!e.tracker_initialized) {
-          if (!dev_decide) {
-            std::fill(e.mask.begin(), e.mask.end(), 0);
-            e.reset_mask();
-          }
-          kind[b] = 1;
-          return;
-        }
-        if (!dev_decide) e.reset_mask();
-        int n = 0;
-        for (Feature* f : e.tracks) {
-          prefetch_ahead(e.tracks, (size_t)n, 2);
-          if (n >= max_pts) { overflow = 1; return; }
-          float* p0 = pts0.h + ((size_t)b * max_pts + n) * 2;
-          float* p1 = pts1.h + ((size_t)b * max_pts + n) * 2;
-          p0[0] = (float)f->xp()[0]; p0[1] = (float)f->xp()[1];
-          if (f->pred[0] != -1 && f->pred[1] != -1) {
-            p1[0] = (float)f->pred[0]; p1[1] = (float)f->pred[1];
-            f->pred[0] = f->pred[1] = -1;
-          } else {
-            p1[0] = p0[0]; p1[1] = p0[1];
-          }
-          ++n;
-        }
-        if (n == 0) {  // tracker.cpp:520-523: no swap, re-initialise on the next frame
-          e.tracker_initialized = false;
-          kind[b] = 3;
-          return;
-        }
-        npts.h[b] = n;
-        kind[b] = 2;
+        kind[b] = e.tracker_lk_begin(pts0.h + (size_t)b * max_pts * 2, pts1.h + (size_t)b * max_pts * 2, max_pts);
+        if (kind[b] == Estimator::kTrkOverflow) overflow = 1;
+        if (kind[b] == Estimator::kTrkLK) npts.h[b] = (int)e.tracks.size();
       });
       if (overflow) return fail(XIVO_ERR_STATE, "tracker feature list exceeds max_pts");
       for (int b : act) {
-        if (kind[b] == 1) { det_list.push_back(b); det_budget[b] = est[b]->tc.num_features_max; }
-        else if (kind[b] == 2) lk_list.push_back(b);
+        if (kind[b] == Estimator::kTrkFirst) det_list.push_back(b);
+        else if (kind[b] == Estimator::kTrkLK) lk_list.push_back(b);
         else off_cur.h[b] = ~0ull;
       }
     }
@@ -1117,7 +981,7 @@ class Batch {
       for (int b = 0; b < B; ++b) { tkind.h[b] = 0; fast_off.h[b] = ~0ull; }
       for (int b : act) {
         tkind.h[b] = kind[b];
-        if (kind[b] == 1 || kind[b] == 2) fast_off.h[b] = ((size_t)b * 2 + (1 - prev_slot[b])) * pd.total;
+        if (kind[b] == Estimator::kTrkFirst || kind[b] == Estimator::kTrkLK) fast_off.h[b] = off_cur.h[b];
       }
       HostScope hx("x_i_trk_h2d");
       XB_CUDA(up_blob(tt, tt_up_bytes, st));
@@ -1126,35 +990,18 @@ class Batch {
       if (tma_pyr) { XB_CUDA(ring_img.up(st)); XB_CUDA(pyr_img.up(st)); }
     }
     std::unique_ptr<HostScope> hx_pyr(new HostScope("x_i_trk_pyr"));
-    if (tma_pyr) {
-      ProfScope ps("pyrdown", st);
-      if (int rc = launch_pyrdown_tma(st, tm_ring, ring_img.d, dPyr, 0, off_cur.d, pd, 0, 1, B)) return rc;
-      for (int l = 1; l + 1 < pd.n_levels; ++l) {
-        if (tm_lvl_ok[l]) { if (int rc = launch_pyrdown_tma(st, tm_lvl[l], pyr_img.d, dPyr, 0, off_cur.d, pd, l, 0, B)) return rc; }
-        else if (int rc = launch_pyrdown_level(st, dPyr, 0, off_cur.d, pd, B, nullptr, l)) return rc;
-      }
-    } else if (int rc = launch_build_pyramid(st, dPyr, 0, off_cur.d, pd, B, frame_ptr.d)) return rc;
-    g_launches += std::max(1, pd.n_levels - 1);
+    if (int rc = build_pyramids(true)) return rc;
     hx_pyr.reset();
     {
       int nact = 0;
       for (int b = 0; b < B; ++b) nact += off_cur.h[b] != ~0ull;
       Prof::get().add_work("pyrdown", nact * (7.0 / 3.0) * rows * cols * cn);  // SURVEY.md §8d: (7/3) W H c bytes
     }
-    if (dev_decide) return tracker_decide_on_device(act, lk_list, det_list, kind, &hs_issue);
+    if (dev_decide) return tracker_decide_on_device(act, lk_list, kind, &hs_issue);
     hs_issue.reset();
     if (!lk_list.empty()) {
       XB_CUDA(pts0.up(st)); XB_CUDA(pts1.up(st));
-      const TrackerCfg& tc = est[0]->tc;
-      if (int rc = launch_lk_track(st, dPyr, dPyr, 0, off_prev.d, off_cur.d, pd, pts0.d, pts1.d, lkst.d, lkerr.d, npts.d, max_pts, B,
-                                   tc.win_size, tc.max_iter, tc.eps, 1, 1e-4))
-        return rc;
-      g_launches += 1;
-      {
-        double np_ = 0;
-        for (int b : lk_list) np_ += npts.h[b];
-        Prof::get().add_work("lk_track", np_ * pd.n_levels * (17.0 * 17.0 + 25.0 * 25.0) * cn);  // §8d: L (17^2+25^2) c bytes / feature
-      }
+      if (int rc = track_lk(lk_list)) return rc;
       XB_CUDA(pts1.down(st)); XB_CUDA(lkst.down(st));
       if (desc_on) {  // descriptors at the tracked positions (tracker.cpp:530-545), same stream, same wait
         if (int rc = launch_brief(st, dPyr, 0, off_cur.d, rows, cols, cn, pts1.d, npts.d, max_pts, descT.d, validT.d, B)) return rc;
@@ -1163,221 +1010,68 @@ class Batch {
       }
       { HostScope hw("wait_lk"); if (int rc = wait(st)) return rc; }
       HostScope hs("tracker_accept");
-      std::vector<int> need(B, 0);
       pfor(lk_list, [&](int b, int) {
         HostScope hx("x_trk_accept");
-        Estimator& e = *est[b];
-        int i = 0, num_valid = 0, num_failed = 0;
-        static thread_local std::vector<uint8_t> stat;  // cv status vector of this frame (tracker.cpp:501, :573-591)
-        stat.assign(e.tracks.size(), 0);
-        if (desc_on) {  // tracker.cpp:546-565: keypoints the extractor dropped (border band) are skipped; a distant descriptor forces a drop
-          int j = 0;
-          for (Feature* f : e.tracks) {
-            const size_t k = (size_t)b * max_pts + j++;
-            if (!validT.h[k]) continue;
-            const uint8_t* dnew = descT.h + k * 32;
-            if (e.tc.descriptor_distance_thresh != -1) {
-              int dist = 0;
-              for (int q = 0; q < 32; ++q) dist += __builtin_popcount((unsigned)(f->descriptor[q] ^ dnew[q]));
-              if (dist > e.tc.descriptor_distance_thresh) lkst.h[k] = 0;  // enforce to be dropped
-              else if (e.tc.differential) memcpy(f->descriptor, dnew, 32);
-            } else if (e.tc.differential) {
-              memcpy(f->descriptor, dnew, 32);
-            }
-          }
-        }
-        for (Feature* f : e.tracks) {
-          const float* p1 = pts1.h + ((size_t)b * max_pts + i) * 2;
-          bool ok = lkst.h[(size_t)b * max_pts + i] != 0;
-          if (ok) {
-            const double dx = f->xp()[0] - (double)p1[0], dy = f->xp()[1] - (double)p1[1];
-            if (e.mask_valid(p1[0], p1[1]) && std::sqrt(dx * dx + dy * dy) < e.tc.max_pixel_displacement) {
-              f->tstatus = TrackStatus::TRACKED;
-              f->observe((double)p1[0], (double)p1[1]);
-              e.mask_out(p1[0], p1[1]);
-              ++num_valid;
-            } else {
-              ok = false;
-            }
-          }
-          stat[i] = ok;
-          if (!ok) ++num_failed;
-          ++i;
-        }
-        e.num_new_detections = 0;
-        e.num_failed_to_track = num_failed;
-        bool or_done = false;
-        if (e.tc.do_outlier_rejection) {
-          // Tracker::OutlierRejection (tracker.cpp:594-599, :705-753): homography outliers lose their status after their track and the
-          // mask were updated; pts0 / pts1 are this frame's LK input and output (cv::Point2f)
-          or_done = homography::tracker_outlier_rejection(pts0.h + (size_t)b * max_pts * 2, pts1.h + (size_t)b * max_pts * 2, (int)e.tracks.size(), stat,
-                                                          e.tc.outlier_method, e.tc.outlier_reproj_thresh, e.tc.outlier_max_iters, e.tc.outlier_confidence,
-                                                          &e.num_outliers_rejected);
-          num_valid -= e.num_outliers_rejected;
-        }
-        check_h[b] = or_done && e.tc.do_outlier_rejection;
-        i = 0;
-        if (desc_on) query_feats[b].clear();
-        for (Feature* f : e.tracks)
-          if (!stat[i++]) {
-            f->tstatus = TrackStatus::DROPPED;  // (with the rescue path the reference marks them after DetectLK: the same final state)
-            if (desc_on) query_feats[b].push_back(f);  // newly_dropped_tracks (tracker.cpp:601-608)
-          }
-        if (num_valid < e.tc.num_features_min) need[b] = e.tc.num_features_max - num_valid;
+        const size_t r = (size_t)b * max_pts;
+        est[b]->tracker_lk_accept(pts0.h + 2 * r, pts1.h + 2 * r, lkst.h + r, desc_on ? descT.h + 32 * r : nullptr, desc_on ? validT.h + r : nullptr);
       });
       for (int b : lk_list)
-        if (need[b] > 0) { det_list.push_back(b); det_budget[b] = need[b]; }
+        if (est[b]->detect_budget > 0) det_list.push_back(b);
     }
     if (!det_list.empty()) {
       // FAST on the current level-0 image of the sequences that need new features
       for (int b = 0; b < B; ++b) off_prev.h[b] = ~0ull;  // reuse off_prev as the FAST selector
-      for (int b : det_list) off_prev.h[b] = ((size_t)b * 2 + (1 - prev_slot[b])) * pd.total;
+      for (int b : det_list) off_prev.h[b] = off_cur.h[b];
       XB_CUDA(off_prev.up(st));
-      const TrackerCfg& tc = est[0]->tc;
-      if (int rc = launch_fast_detect(st, dPyr, 0, off_prev.d, rows, cols, cn, tc.fast_threshold, tc.fast_nonmax, kp.d, max_kp, kpcount.d, B, nullptr,
-                                      tma_fast ? &tm_fast : nullptr, pd.total))
-        return rc;
-      g_launches += 1;
+      if (int rc = detect_and_fetch(det_list, off_prev.d)) return rc;
       Prof::get().add_work("fast_detect", det_list.size() * 2.0 * rows * cols);  // §8d: 2 W H bytes
-      XB_CUDA(kpcount.down(st));
-      { HostScope hw("wait_fastcount"); if (int rc = wait(st)) return rc; }
-      for (int b : det_list) {
-        const int n = std::min(kpcount.h[b], max_kp);
-        if (n) { Prof::get().d2h += sizeof(unsigned) * n; XB_CUDA(cudaMemcpyAsync(kp.h + (size_t)b * max_kp, kp.d + (size_t)b * max_kp, sizeof(unsigned) * n, cudaMemcpyDeviceToHost, st)); }
-      }
-      { HostScope hw("wait_fastkp"); if (int rc = wait(st)) return rc; }
       if (desc_on) {  // DetectLK with descriptors: every masked keypoint gets one, dropped tracks may claim a keypoint (tracker.cpp:231-327)
-        pfor(det_list, [&](int b, int) { order_keypoints(b, kp.h + (size_t)b * max_kp, std::min(kpcount.h[b], max_kp), true); });
-        if (!est[0]->tc.match_dropped_tracks)
-          for (int b : det_list) query_feats[b].clear();
+        pfor(det_list, [&](int b, int) {
+          nkps.h[b] = est[b]->tracker_order_keypoints(kp.h + (size_t)b * max_kp, std::min(kpcount.h[b], max_kp), true, kpxy.h + (size_t)b * max_kp * 2);
+        });
         if (int rc = describe_and_match(det_list, off_prev.d)) return rc;
         HostScope hs("tracker_select");
         pfor(det_list, [&](int b, int) {
-          detect_select_desc(b, det_budget[b], check_h[b] != 0);
-          est[b]->tracker_initialized = true;
+          std::vector<std::array<int, 3>> m;
+          matches_of(b, &m);
+          est[b]->tracker_detect_select_desc(descK.h + (size_t)b * max_kp * 32, m);
         });
       } else {
         HostScope hs("tracker_select");
         pfor(det_list, [&](int b, int) {
           HostScope hx("x_trk_select");
-          Estimator& e = *est[b];
-          detect_select(e, kp.h + (size_t)b * max_kp, std::min(kpcount.h[b], max_kp), det_budget[b]);
-          e.tracker_initialized = true;
+          est[b]->tracker_detect_select(kp.h + (size_t)b * max_kp, std::min(kpcount.h[b], max_kp));
         });
       }
     }
-    if (desc_on)  // tracker.cpp:617-619: every newly dropped track ends DROPPED, "rescued" or not (DetectLK worked on a copy of the vector)
-      for (int b : lk_list)
-        for (Feature* f : query_feats[b]) f->tstatus = TrackStatus::DROPPED;
-    for (int b : act)
-      if (off_cur.h[b] != ~0ull) prev_slot[b] = 1 - prev_slot[b];  // std::swap(pyramid, pyramid_)
+    for (int b : lk_list) est[b]->tracker_lk_finish();
+    swap_pyramids(act);
     return 0;
   }
 
   // Tracker::UpdateMatch (tracker.cpp:341-460): detect without a mask, describe, cross-checked nearest-neighbour matching of the existing
-  // features' descriptors against the new keypoints (device), checks + optional homography rejection, unmatched features dropped,
-  // unmatched keypoints become features (host).
+  // features' descriptors against the new keypoints (device); the decisions are the estimators' (tracker_host.cpp.inc).
   int tracker_update_match(const std::vector<int>& act, const std::vector<int>& slots) {
     cudaStream_t st = st1;
-    const size_t ib = (size_t)rows * cols * cn;
-    const TrackerCfg& tc = est[0]->tc;
-    for (int b = 0; b < B; ++b) { off_cur.h[b] = ~0ull; off_prev.h[b] = 0; npts.h[b] = 0; }
-    {
-      std::vector<char> seen(ring_n, 0);
-      for (int k : slots)
-        if (!seen[k]) { seen[k] = 1; XB_CUDA(cudaStreamWaitEvent(st, ring_ev[k], 0)); }
-    }
-    for (size_t i = 0; i < act.size(); ++i) {
-      const int b = act[i];
-      const int cur = 1 - prev_slot[b];
-      off_cur.h[b] = ((size_t)b * 2 + cur) * pd.total;
-      frame_ptr.h[b] = dRing + ((size_t)b * ring_n + slots[i]) * ib;
-      if (tma_pyr) { ring_img.h[b] = b * ring_n + slots[i]; pyr_img.h[b] = b * 2 + cur; }
-    }
+    if (int rc = begin_frame(act, slots)) return rc;
     XB_CUDA(off_cur.up(st)); XB_CUDA(frame_ptr.up(st));
     if (tma_pyr) { XB_CUDA(ring_img.up(st)); XB_CUDA(pyr_img.up(st)); }
-    // the frame enters through the pyramid's ingest pass (level 0 of the current pyramid is the image the detector and the extractor read)
-    if (tma_pyr) { if (int rc = launch_pyrdown_tma(st, tm_ring, ring_img.d, dPyr, 0, off_cur.d, pd, 0, 1, B)) return rc; }
-    else if (int rc = launch_pyrdown_level(st, dPyr, 0, off_cur.d, pd, B, frame_ptr.d, 0)) return rc;
-    if (int rc = launch_fast_detect(st, dPyr, 0, off_cur.d, rows, cols, cn, tc.fast_threshold, tc.fast_nonmax, kp.d, max_kp, kpcount.d, B, nullptr,
-                                    tma_fast ? &tm_fast : nullptr, pd.total))
-      return rc;
-    g_launches += 2;
-    XB_CUDA(kpcount.down(st));
-    { HostScope hw("wait_fastcount"); if (int rc = wait(st)) return rc; }
-    for (int b : act) {
-      const int n = std::min(kpcount.h[b], max_kp);
-      if (n) XB_CUDA(cudaMemcpyAsync(kp.h + (size_t)b * max_kp, kp.d + (size_t)b * max_kp, sizeof(unsigned) * n, cudaMemcpyDeviceToHost, st));
-    }
-    { HostScope hw("wait_fastkp"); if (int rc = wait(st)) return rc; }
+    if (int rc = build_pyramids(false)) return rc;
+    if (int rc = detect_and_fetch(act, off_cur.d)) return rc;
     std::atomic<int> overflow{0};
     pfor(act, [&](int b, int) {
       Estimator& e = *est[b];
-      order_keypoints(b, kp.h + (size_t)b * max_kp, std::min(kpcount.h[b], max_kp), false);
-      query_feats[b].clear();
-      if (e.tracker_initialized) query_feats[b].assign(e.tracks.begin(), e.tracks.end());
-      if ((int)query_feats[b].size() > max_pts) overflow = 1;
+      nkps.h[b] = e.tracker_match_begin(kp.h + (size_t)b * max_kp, std::min(kpcount.h[b], max_kp), kpxy.h + (size_t)b * max_kp * 2);
+      if ((int)e.query_feats.size() > max_pts) overflow = 1;
     });
     if (overflow) return fail(XIVO_ERR_STATE, "tracker feature list exceeds max_pts");
     if (int rc = describe_and_match(act, off_cur.d)) return rc;
     pfor(act, [&](int b, int) {
-      Estimator& e = *est[b];
-      const std::vector<unsigned>& v = sorted_kp[b];
-      const uint8_t* D = descK.h + (size_t)b * max_kp * 32;
-      const std::vector<Feature*>& feats = query_feats[b];
-      std::vector<char> kp_matched(v.size(), 0), feat_matched(feats.size(), 0);
-      e.num_new_detections = 0;
-      if (e.tracker_initialized) {
-        std::vector<std::array<int, 3>> m;
-        if (nq.h[b] && !v.empty()) cross_checked(b, &m);
-        std::vector<uint8_t> mstat(m.size(), 0);
-        int zeros = 0;
-        for (size_t i = 0; i < m.size(); ++i) {
-          Feature* f = feats[m[i][0]];
-          const double x = (v[m[i][1]] >> 8) & 0xfff, y = v[m[i][1]] >> 20;
-          const bool ok_desc = e.tc.descriptor_distance_thresh > 0 ? m[i][2] < e.tc.descriptor_distance_thresh : true;
-          const double dx = x - f->xp()[0], dy = y - f->xp()[1];
-          mstat[i] = ok_desc && std::sqrt(dx * dx + dy * dy) < e.tc.max_pixel_displacement;
-          zeros += !mstat[i];
-        }
-        e.num_failed_to_track = (int)feats.size() - (int)m.size() + zeros;
-        if (e.tc.do_outlier_rejection && !m.empty()) {  // pts0 = the features' creation keypoints, pts1 = the matched new keypoints (tracker.cpp:398-408)
-          std::vector<float> p0(2 * m.size()), p1(2 * m.size());
-          for (size_t i = 0; i < m.size(); ++i) {
-            p0[2 * i] = feats[m[i][0]]->kp0[0]; p0[2 * i + 1] = feats[m[i][0]]->kp0[1];
-            p1[2 * i] = (float)((v[m[i][1]] >> 8) & 0xfff); p1[2 * i + 1] = (float)(v[m[i][1]] >> 20);
-          }
-          homography::tracker_outlier_rejection(p0.data(), p1.data(), (int)m.size(), mstat, e.tc.outlier_method, e.tc.outlier_reproj_thresh, e.tc.outlier_max_iters,
-                                                e.tc.outlier_confidence, &e.num_outliers_rejected);
-        }
-        for (size_t i = 0; i < m.size(); ++i) {
-          if (!mstat[i]) continue;
-          kp_matched[m[i][1]] = 1; feat_matched[m[i][0]] = 1;
-          Feature* f = feats[m[i][0]];
-          f->observe((double)((v[m[i][1]] >> 8) & 0xfff), (double)(v[m[i][1]] >> 20));
-          if (e.tc.differential) memcpy(f->descriptor, D + 32 * (size_t)m[i][1], 32);
-          f->tstatus = TrackStatus::TRACKED;
-        }
-      }
-      int dropped = 0;
-      for (size_t i = 0; i < feats.size(); ++i)
-        if (!feat_matched[i]) { feats[i]->tstatus = TrackStatus::DROPPED; ++dropped; }
-      // (before the first frame features_ is empty: everything detected is new)
-      int to_create = e.tc.num_features_max - (int)e.tracks.size() + (e.tracker_initialized ? dropped : 0);
-      for (size_t i = 0; i < v.size() && to_create > 0; ++i) {
-        if (kp_matched[i]) continue;
-        Feature* f = e.create_feature((double)((v[i] >> 8) & 0xfff), (double)(v[i] >> 20));
-        if (!f) return;
-        f->response = (float)(v[i] & 0xff);
-        memcpy(f->descriptor, D + 32 * i, 32);
-        f->has_descriptor = true;
-        e.tracks.push_back(f);
-        e.num_new_detections++;
-        --to_create;
-      }
-      e.tracker_initialized = true;
+      std::vector<std::array<int, 3>> m;
+      matches_of(b, &m);
+      est[b]->tracker_match_finish(descK.h + (size_t)b * max_kp * 32, m);
     });
-    for (int b : act) prev_slot[b] = 1 - prev_slot[b];
+    swap_pyramids(act);
     return 0;
   }
 

@@ -431,6 +431,27 @@ class Estimator {
   void update_step_after_gate_finish();
   void update_step_after_update(const double* err, const double* Pmm, const double* diagP, bool had_update);
   void tracker_only_finish();
+  // ---- image tracker (tracker_host.cpp.inc: src/tracker.cpp), split at the device phases.  Arrays are the sequence's own rows of the
+  // read-back tables; keypoints are packed as launch_fast_detect writes them.
+  void tracker_set_geometry(int rows, int cols, bool host_mask);  // host_mask: the mask bitmap exists only on the host-decision path
+  // UpdateLK up to the LK launch: writes p0 / p1 (max_pts rows) and returns the frame's kind
+  enum { kTrkOverflow = -1, kTrkFirst = 1, kTrkLK = 2, kTrkEmpty = 3 };  // (values as track_accept_kernel reads them)
+  int tracker_lk_begin(float* p0, float* p1, int max_pts);
+  // UpdateLK's descriptor check, accept loop and homography rejection (desc / desc_valid: BRIEF at p1, null without descriptors);
+  // returns the detection budget
+  int tracker_lk_accept(const float* p0, const float* p1, uint8_t* lkst, const uint8_t* desc, const uint8_t* desc_valid);
+  // DetectLK's greedy pick: without descriptors from the detected keypoints; with descriptors from sorted_kp (tracker_order_keypoints),
+  // their descriptors and the cross-checked (query, keypoint, distance) matches of query_feats
+  void tracker_detect_select(const unsigned* kps, int n);
+  void tracker_detect_select_desc(const uint8_t* desc, const std::vector<std::array<int, 3>>& matches);
+  void tracker_lk_finish();
+  // keypoints in the order DetectLK / UpdateMatch walk them, into sorted_kp and kpxy (x, y per keypoint); returns their count
+  int tracker_order_keypoints(const unsigned* kps, int n, bool use_mask, float* kpxy);
+  // UpdateLK with the decisions made on the device: the accept kernel's keep flags, the select kernel's picks
+  void tracker_replay(int kind, const float* p1, const uint8_t* keep, int need, const unsigned* picks, int npicks);
+  // UpdateMatch: keypoint order and query list before the device phase, the matches applied after it
+  int tracker_match_begin(const unsigned* kps, int n, float* kpxy);
+  void tracker_match_finish(const uint8_t* desc, const std::vector<std::array<int, 3>>& matches);
 
   // helpers used by Batch
   EkfLayout lay;
@@ -506,6 +527,10 @@ class Estimator {
   int rows = 0, cols = 0;
   int num_failed_to_track = 0, num_new_detections = 0, num_mh_rejected = 0;
   int num_outliers_rejected = 0;  // Tracker::num_outliers_rejected_ (keeps its last value when OutlierRejection returns early, tracker.cpp:598, :713-715)
+  std::vector<unsigned> sorted_kp;      // this frame's detected keypoints in selection order (tracker_order_keypoints)
+  std::vector<Feature*> query_feats;    // the features whose descriptors are matched against sorted_kp
+  int detect_budget = 0;                // DetectLK's num_to_add of this frame (0: no detection)
+  bool check_homography = false;        // DetectLK's check_homography: this frame's outlier rejection ran
   int num_depth_refined = 0, num_depth_refine_failed = 0;
   int num_good_triangulations = 0, num_bad_triangulations = 0;  // Feature::num_good/bad_triangulations_ (feature.cpp:730-748)
   // time / imu (src/estimator.cpp)
@@ -526,6 +551,8 @@ class Estimator {
   void reset_mask();
   void mask_out(double x, double y);
   bool mask_valid(double x, double y) const;
+  Feature* track_keypoint(unsigned k, const uint8_t* desc);           // a detected keypoint becomes a new track (desc: its descriptor or null)
+  bool match_passes(const Feature* f, unsigned k, int dist) const;    // CheckDescriptorDistance + displacement of a cross-checked match
 
  private:
   std::vector<Msg> buf_;
@@ -580,5 +607,9 @@ class Estimator {
 // The first setting that one batch handle needs to be the same for every sequence and that differs between the two estimators,
 // as its config key ("tracker_cfg.KLT.win_size"), or "" when a sequence configured like `b` may join a handle configured like `a`.
 std::string batch_incompatibility(const Estimator& a, const Estimator& b);
+
+// cv::BFMatcher's cross-checked matches (knnMatch with compactResult, in query order) as (query, keypoint, distance), from the nearest
+// keypoint of every query (best_t / best_t_dist) and the nearest query of every keypoint (best_q)
+void cross_checked(int nq, const int* best_t, const int* best_t_dist, const int* best_q, std::vector<std::array<int, 3>>* out);
 
 }  // namespace xb

@@ -28,6 +28,10 @@ int launch_fast_detect(cudaStream_t st, const uint8_t* img, unsigned long long i
                        int rows, int cols, int cn, int thr, int nonmax, unsigned* kp_out, int max_kp, int* kp_count, int batch,
                        const int* need = nullptr, const CUtensorMap* tma_map = nullptr, unsigned long long tma_img_stride = 0,
                        bool count_is_zero = false /*kp_count was cleared by an earlier kernel of the stream (track_accept)*/);
+// A keypoint of launch_fast_detect is packed as y << 20 | x << 8 | score: ascending order is raster order within a score.
+inline int kp_x(unsigned k) { return (k >> 8) & 0xfff; }
+inline int kp_y(unsigned k) { return k >> 20; }
+inline int kp_score(unsigned k) { return k & 0xff; }
 // Descriptor path (tracker.cpp:231-292, :341-460, :530-565): BRIEF-32 at given keypoints (kp_xy: batch x max_kp x 2 floats, nkp: batch counts;
 // desc: batch x max_kp x 32 bytes, valid: 0 for keypoints closer than 28 px to the border) and, for the cross-checked brute-force matcher,
 // the nearest descriptor of side b for every descriptor of side a (index and Hamming distance; -1 when b is empty; first index on ties).

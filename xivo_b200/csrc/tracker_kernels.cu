@@ -1310,7 +1310,7 @@ int launch_hamming_nearest(cudaStream_t st, const uint8_t* a, const int* na, int
 // (tracker.cpp:224-229, :295-328) without a host round trip.  Both walk a list in order while a mask of claimed pixels grows, so each
 // sequence is one CTA whose warp 0 does the sequential walk (the 15 x 15 mask-out of one feature is spread over the lanes);
 // the mask lives in shared memory as a bitmap (bit = pixel still free).  Same arithmetic as the host code they replace
-// (estimator_host.cpp.inc: mask_out / mask_valid; estimator.cu: detect_select): truncation for the validity test, round-half-even
+// (estimator_host.cpp.inc: mask_out / mask_valid; tracker_host.cpp.inc: Estimator::tracker_detect_select): truncation for the validity test, round-half-even
 // for the block corners, the displacement test in double precision.
 // ------------------------------------------------------------------------------------------
 __device__ __forceinline__ void mask_reset(unsigned* m, int stride, const TrackDecideCfg& c, int tid, int nthr) {
