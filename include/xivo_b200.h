@@ -179,6 +179,22 @@ int xivo_oos_project(xivo_ctx* ctx, int G, int F, const double* camera, const do
 int xivo_find_homography_mask(const float* pts0, const float* pts1, int n, int method, double reproj_thresh, int max_iters,
                               double confidence, uint8_t* mask, int* ok);
 
+/* PNG frames, decoded as cv::imread decodes them for the reference (pybind11/pyxivo.cpp:81-85, :119-123; src/app/vio.cpp:72).
+ * Accepted: colour types 0 (grey), 2 (RGB), 4 (grey + alpha), 6 (RGBA) at 8 or 16 bits, not interlaced.  Refused with XIVO_ERR_ARG
+ * and the reason in xivo_last_error(): palette images, bit depths 1/2/4, Adam7 interlace, a bad signature, a missing or misplaced
+ * IHDR, a missing IDAT or IEND, a chunk running past the end of the data, zero or oversized (> 16384 px a side) dimensions.
+ * Ancillary chunks (gAMA, sRGB, tRNS, tEXt, ...) are skipped, as imread's colour and grey outputs ignore them.  The zlib header and
+ * Adler-32 are checked and the inflated length must equal rows x (1 + cols x bytes per pixel); chunk CRCs are not checked (libpng
+ * checks them).
+ *
+ * xivo_png_info: host-only container walk, no context.  channels = samples per pixel of the file (1, 2, 3, 4), bit_depth 8 or 16. */
+int xivo_png_info(const uint8_t* png, size_t n, int* rows, int* cols, int* channels, int* bit_depth);
+/* Decodes n PNGs of any geometry in one launch pair (png_inflate_kernel, png_unfilter_kernel) into host buffers out[i] of
+ * rows x cols x channels bytes.  channels = 3: cv::imread(path) (IMREAD_COLOR): BGR, grey replicated, alpha stripped, 16-bit samples
+ * keep their high byte.  channels = 1: IMREAD_GRAYSCALE of grey and grey + alpha files (colour files are refused).  If any frame
+ * fails, nothing is written and XIVO_ERR_ARG names the frame index and the reason. */
+int xivo_decode_png(xivo_ctx* ctx, int n, const uint8_t* const* png, const size_t* png_bytes, int channels, uint8_t* const* out);
+
 /* Covariance slot surgery; replaces AddGroupToState / AddFeatureToState+FillCovarianceBlock /
  * RemoveGroupFromState / RemoveFeatureFromState / FixFeatureXY / SwitchRefGroup
  * (src/estimator.cpp:739-846, :1362-1391, :1474-1478, src/feature.cpp:753-776).

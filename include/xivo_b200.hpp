@@ -82,6 +82,10 @@ class Estimator {
   }
   void VisualMeas(const timestamp_t& ts, const ImageView& img) { visual(ts, img, 0); }
   void VisualMeasTrackerOnly(const timestamp_t& ts, const ImageView& img) { visual(ts, img, 1); }
+  // cv::imread(path) + VisualMeas, the overloads of the reference's binding (pybind11/pyxivo.cpp:338-341) and its vio app
+  // (src/app/vio.cpp:72): the PNG file is decoded on the device into the frame ring like IMREAD_COLOR (xivo_batch_visual_meas_png, BGR)
+  void VisualMeas(const timestamp_t& ts, const std::string& path) { visual_png(ts, path, 0); }
+  void VisualMeasTrackerOnly(const timestamp_t& ts, const std::string& path) { visual_png(ts, path, 1); }
   // xp_and_depths: n x 3 row-major (x, y, depth), as MatX3 rows in the reference
   void VisualMeasPointCloud(const timestamp_t& ts, const std::vector<int>& feature_ids, const std::vector<double>& xp_and_depths) {
     pointcloud(ts, feature_ids, xp_and_depths, 0);
@@ -221,6 +225,15 @@ class Estimator {
     const uint64_t t = (uint64_t)ts.count();
     const uint8_t* p = img.data;
     check(xivo_batch_visual_meas(b_, &t, &p, img.rows, img.cols, img.channels, tracker_only));
+  }
+  void visual_png(const timestamp_t& ts, const std::string& path, int tracker_only) {
+    std::ifstream f(path, std::ios::binary);
+    if (!f) throw Error(XIVO_ERR_ARG, "cannot open " + path);
+    const std::vector<uint8_t> bytes((std::istreambuf_iterator<char>(f)), std::istreambuf_iterator<char>());
+    const uint64_t t = (uint64_t)ts.count();
+    const uint8_t* src = bytes.data();
+    const size_t n = bytes.size();
+    if (int rc = xivo_batch_visual_meas_png(b_, &t, &src, &n, 3, tracker_only)) throw Error(rc, path + ": " + xivo_last_error());
   }
   void pointcloud(const timestamp_t& ts, const std::vector<int>& ids, const std::vector<double>& xpd, int tracker_only) {
     if (xpd.size() != 3 * ids.size()) throw Error(XIVO_ERR_ARG, "xp_and_depths must be n x 3");

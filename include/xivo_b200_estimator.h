@@ -47,6 +47,18 @@ int xivo_batch_inertial_meas(xivo_batch* b, const uint64_t* ts_ns, const double*
 int xivo_batch_visual_meas(xivo_batch* b, const uint64_t* ts_ns, const uint8_t* const* imgs, int rows, int cols,
                            int channels, int tracker_only);
 
+/* xivo_batch_visual_meas with the frames given as PNG files (png[s]: png_bytes[s] bytes), decoded on the device the way cv::imread(path)
+ * decodes them for the reference (pybind11/pyxivo.cpp:81-85, src/app/vio.cpp:72; formats and refusals: xivo_decode_png in xivo_b200.h).
+ * channels = 3: the BGR imread result; 1: the grey sample of grey / grey + alpha files.  Every frame must have the batch geometry and
+ * camera_cfg rows / cols (same checks as xivo_batch_visual_meas); colour type and bit depth may differ between sequences and frames.
+ * The host walks the chunks and packs the image data of all sequences into one pinned upload; png_inflate_kernel and png_unfilter_kernel
+ * decode it straight into the frame-ring slots the tracker reads.  A refused frame (container refusal on the host, corrupt deflate data,
+ * Adler-32 or length mismatch on the device) returns XIVO_ERR_ARG naming the frame and the reason before any message is pushed: no
+ * sequence changes and the handle stays usable.  The caller's buffers are free when the call returns.  Pending
+ * xivo_batch_prefetch_frames uploads are dropped, as for any call with other buffers. */
+int xivo_batch_visual_meas_png(xivo_batch* b, const uint64_t* ts_ns, const uint8_t* const* png, const size_t* png_bytes, int channels,
+                               int tracker_only);
+
 /* Same, with the frames already resident in device memory (imgs_dev[s] are device pointers on this
  * context's GPU); used to measure the device-resident throughput. */
 int xivo_batch_visual_meas_device(xivo_batch* b, const uint64_t* ts_ns, const uint8_t* const* imgs_dev, int rows, int cols,

@@ -10,6 +10,7 @@
 #include <cstdint>
 #include <cstdio>
 #include <fstream>
+#include <iterator>
 #include <memory>
 #include <sstream>
 #include <stdexcept>
@@ -34,6 +35,13 @@ struct IMU : Message {
   }
 };
 }  // namespace msg
+
+// whole file as bytes (the PNG frames handed to Estimator::VisualMeas(ts, path) / xivo_decode_png)
+inline std::vector<uint8_t> ReadFileBytes(const std::string& path) {
+  std::ifstream f(path, std::ios::binary);
+  if (!f) throw std::runtime_error("cannot open " + path);
+  return std::vector<uint8_t>((std::istreambuf_iterator<char>(f)), std::istreambuf_iterator<char>());
+}
 
 class DataLoader {
  public:

@@ -19,6 +19,7 @@ SOURCES = [
     ("ekf_kernels.cu", []),
     ("ekf_tc_kernels.cu", []),
     ("capi.cu", []),
+    ("png_kernels.cu", []),
     # host state machine: AVX2/FMA for the 23x23 integrator loops (results within 1e-16 relative)
     ("estimator.cu", ["-Xcompiler", "-march=x86-64-v3"]),
 ]

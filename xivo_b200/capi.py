@@ -59,6 +59,14 @@ def launch_count() -> int:
     return int(lib().xivo_launch_count())
 
 
+def png_info(data: bytes):
+    """xivo_png_info: (rows, cols, channels, bit_depth) of a PNG file's bytes; XivoError names the reason for a refused file."""
+    data = bytes(data)
+    r, c, ch, bd = C.c_int(), C.c_int(), C.c_int(), C.c_int()
+    _check(lib().xivo_png_info(C.c_char_p(data), C.c_size_t(len(data)), C.byref(r), C.byref(c), C.byref(ch), C.byref(bd)), "xivo_png_info")
+    return r.value, c.value, ch.value, bd.value
+
+
 class Context:
     """xivo_ctx: one CUDA device + stream."""
 
@@ -134,6 +142,23 @@ class Context:
             "xivo_lk_track",
         )
         return p1, st, er
+
+    def decode_png(self, blobs, channels=3):
+        """xivo_decode_png: PNG files' bytes (any geometry) -> list of rows x cols x 3 (BGR, cv2.imread) or rows x cols (grey) uint8."""
+        blobs = [bytes(b) for b in blobs]
+        n = len(blobs)
+        outs = []
+        for i, b in enumerate(blobs):
+            try:
+                r, c, _, _ = png_info(b)  # the output geometry; xivo_decode_png walks the same chunks again
+            except XivoError as e:
+                raise XivoError(f"png frame {i}: {e}") from None
+            outs.append(np.zeros((r, c, channels) if channels == 3 else (r, c), np.uint8))
+        src = (C.c_char_p * max(n, 1))(*blobs)
+        sizes = (C.c_size_t * max(n, 1))(*[len(b) for b in blobs])
+        dst = (C.c_void_p * max(n, 1))(*[o.ctypes.data for o in outs])
+        _check(lib().xivo_decode_png(self._h, n, src, sizes, int(channels), dst), "xivo_decode_png")
+        return outs
 
     # ------------------------------------------------------------------ EKF
     def jacobian_batch(self, G, F, camera, X24, groups, feat_x, feat_xp, feat_ref, feat_sind, P=None, R=1.0, dense=True):

@@ -15,6 +15,7 @@
 #include "ctx.h"
 #include "estimator.h"
 #include "homography.h"
+#include "png.cuh"
 #include "prof.h"
 #include "workpool.h"
 
@@ -223,7 +224,7 @@ class Batch {
   Json cfg0;                // the creation config: what a reset sequence gets when it is given none
   bool sim_depths = false;  // xivo_init_with_sim_depths was called: a reset sequence inherits it
   unsigned reset_busy = 0;  // st2 ticket after which the host mirrors of the last reset's uploads may be rewritten (0 = free)
-  StreamTicket tk1, tk2;    // completion flags of st1 / st2
+  StreamTicket tk1, tk2, tkc;  // completion flags of st1 / st2 / st_copy
   // The covariance side (IMU propagation, slot edits, Jacobians, update) runs on its own stream so that it
   // overlaps the image tracker's kernels and host phases, which use ctx->stream.
   cudaStream_t st2 = nullptr;
@@ -238,6 +239,11 @@ class Batch {
   uint8_t* dRing = nullptr;   // B x ring_n x img_bytes
   uint8_t* dPyr = nullptr;    // B x 2 x pd.total
   std::vector<int> ring_next, prev_slot;
+  // xivo_batch_visual_meas_png: pinned staging [frame table | IDAT payloads] + its device copy, the decoder's scratch of filtered scanlines
+  // and the per-frame status words; all grown on demand to what a call needs
+  Mirror<unsigned char> png_stage;
+  DevBuf<uint8_t> png_scratch;
+  Mirror<int> png_status;
   // xivo_batch_prefetch_frames: host pointers and ring slots of the frames whose upload is already in flight on st_copy
   struct Prefetched { std::vector<const uint8_t*> ptr; std::vector<int> slot; };
   std::deque<Prefetched> pref;  // oldest first; at most two (the frame about to be consumed and the one after it)
@@ -295,7 +301,7 @@ class Batch {
               cudaMalloc(reinterpret_cast<void**>(&dErr), sizeof(double) * B * N) == cudaSuccess &&
               cudaMalloc(reinterpret_cast<void**>(&dJac), sizeof(FeatJac) * B * lay.F) == cudaSuccess;
     ok = ok && cam.alloc(B) && R.alloc(B) && mh.alloc((size_t)B * lay.F + (size_t)B * N) && pack.alloc((size_t)B * (2 * N + 529)) && sub_out.alloc((size_t)B * max_sub) &&
-         icst.alloc(B) && pmm0.alloc((size_t)B * 529) && tk1.alloc() && tk2.alloc();
+         icst.alloc(B) && pmm0.alloc((size_t)B * 529) && tk1.alloc() && tk2.alloc() && tkc.alloc();
     if (ok) {  // the per-phase upload blobs and the table views inside them
       struct Carve {
         size_t off = 0;
@@ -435,7 +441,8 @@ class Batch {
     for (void* p : {(void*)dP, (void*)dHP, (void*)dKt, (void*)dErr, (void*)dJac, (void*)dRing, (void*)dPyr, (void*)dKt32, (void*)dHP32, (void*)dP0})
       if (p) cudaFree(p);
     cam.release(); R.release(); mh.release(); pack.release(); sub_out.release(); blobS.release(); blobJ.release(); blobU.release();
-    blobI[0].release(); blobI[1].release(); tk1.release(); tk2.release();
+    blobI[0].release(); blobI[1].release(); tk1.release(); tk2.release(); tkc.release();
+    png_stage.release(); png_status.release(); png_scratch.release();
     icst.release(); pmm0.release(); blobG.release();
     lkerr.release(); lkst.release(); kpcount.release();
     kp.release(); tt.release();
@@ -552,7 +559,7 @@ class Batch {
   // have published.  No CUDA call sits in the loop (a stream query every ~2^16 polls only catches a faulted context).
   int wait(cudaStream_t st) {
     static const bool help = !(getenv("XIVO_HELP") && getenv("XIVO_HELP")[0] == '0');
-    StreamTicket& t = st == st2 ? tk2 : tk1;
+    StreamTicket& t = st == st2 ? tk2 : st == st_copy ? tkc : tk1;
     const unsigned want = ++t.next;
     std::unique_ptr<HostScope> hx_t(new HostScope("x_i_ticket"));
     if (StreamWriteValue32Fn wv = stream_write_value32()) {
@@ -708,6 +715,107 @@ class Batch {
   int ingest_done(const std::vector<int>& slot_of) {
     HostScope hsw("wait_ingest_done");
     for (int k : distinct_slots(slot_of)) XB_CUDA(cudaEventSynchronize(ring_ev[k]));
+    return 0;
+  }
+
+  // PNG frames (xivo_batch_visual_meas_png): the host walks the chunks of every sequence's file and packs the IDAT payloads of all of them,
+  // with one PngFrameDesc per frame, into the pinned staging blob (in parallel on the worker pool); ONE upload on st_copy, then
+  // png_inflate_kernel + png_unfilter_kernel decode straight into the ring slots of the frames and ring_ev[slot] is recorded after them,
+  // so the tracker stream orders on the decode like on an upload.  The status words come back on st_copy before any message is pushed:
+  // a refused frame (host- or device-detected) leaves ring_next as the call found it and changes no sequence.  *slot_of = the slots used.
+  int decode_png_frames(const uint8_t* const* png_data, const size_t* png_bytes, int channels, std::vector<int>& slot_of) {
+    std::vector<png::Info> info(B);
+    std::vector<const char*> why(B, nullptr);
+    std::vector<size_t> zlen(B, 0);
+    std::vector<int> all(B);
+    for (int s = 0; s < B; ++s) all[s] = s;
+    {
+      HostScope hp("png_parse");
+      pfor(all, [&](int s, int) {
+        const char* w = "";
+        size_t z = 0;
+        if (png::parse(png_data[s], png_bytes[s], info[s], &w, [&](size_t, size_t len) { z += len; })) why[s] = w;
+        zlen[s] = z;
+      });
+      if (pfor_bad.load()) return fail(XIVO_ERR_STATE, "host state machine threw: " + pfor_msg);
+    }
+    for (int s = 0; s < B; ++s) {
+      if (why[s]) return fail(XIVO_ERR_ARG, "png frame " + std::to_string(s) + ": " + why[s]);
+      if (channels == 1 && info[s].channels > 2)
+        return fail(XIVO_ERR_ARG, "png frame " + std::to_string(s) + ": 1-channel output needs a grey or grey + alpha PNG (colour type " +
+                                      std::to_string(info[s].color_type) + ")");
+      if (info[s].rows != info[0].rows || info[s].cols != info[0].cols)
+        return fail(XIVO_ERR_ARG, "png frame " + std::to_string(s) + " is " + std::to_string(info[s].rows) + " x " + std::to_string(info[s].cols) +
+                                      ", frame 0 is " + std::to_string(info[0].rows) + " x " + std::to_string(info[0].cols) +
+                                      ": all sequences of a batch share one geometry");
+    }
+    if (int rc = ensure_images(info[0].rows, info[0].cols, channels)) return rc;
+    const size_t ib = (size_t)rows * cols * cn;
+    const size_t table = ((size_t)B * sizeof(PngFrameDesc) + 15) & ~(size_t)15;
+    std::vector<size_t> zoff(B);
+    size_t zsum = 0, scratch = 0;
+    for (int s = 0; s < B; ++s) {
+      zoff[s] = zsum;
+      zsum += zlen[s];
+      scratch += (size_t)info[s].raw_bytes();
+    }
+    const size_t stage_bytes = table + zsum;
+    if (png_stage.n < stage_bytes) {  // grown to 1.25 x the need: frames of one sequence compress to similar sizes
+      png_stage.release();
+      if (!png_stage.alloc(stage_bytes + stage_bytes / 4)) return fail(XIVO_ERR_CUDA, "png staging allocation failed");
+    }
+    if (png_scratch.n < scratch) {
+      png_scratch.alloc(scratch + scratch / 4);
+      if (!png_scratch.ok()) return fail(XIVO_ERR_CUDA, "png scratch allocation failed");
+    }
+    if (png_status.n < (size_t)B && !png_status.alloc(B)) return fail(XIVO_ERR_CUDA, "png status allocation failed");
+    // pending prefetches are dropped as for any call with other buffers; ring_next after that is what a refusal restores
+    if (!pref.empty()) {
+      for (int s = 0; s < B; ++s) ring_next[s] = pref.front().slot[s];
+      pref.clear();
+    }
+    const std::vector<int> ring_before = ring_next;
+    fresh_slots(slot_of);
+    PngFrameDesc* fr = reinterpret_cast<PngFrameDesc*>(png_stage.h);
+    {
+      HostScope hk("png_pack");
+      std::vector<size_t> soff(B);
+      size_t so = 0;
+      for (int s = 0; s < B; ++s) { soff[s] = so; so += (size_t)info[s].raw_bytes(); }
+      pfor(all, [&](int s, int) {
+        uint8_t* dst = png_stage.h + table + zoff[s];
+        png::Info I;
+        const char* w = "";
+        png::parse(png_data[s], png_bytes[s], I, &w, [&](size_t off, size_t len) { memcpy(dst, png_data[s] + off, len); dst += len; });
+        PngFrameDesc& d = fr[s];
+        d.in_off = zoff[s];
+        d.in_len = zlen[s];
+        d.scratch_off = soff[s];
+        d.out_off = ((size_t)s * ring_n + slot_of[s]) * ib;
+        d.rows = I.rows;
+        d.cols = I.cols;
+        d.bpp = I.bpp;
+        d.channels = I.channels;
+        d.bps = I.bit_depth / 8;
+        d.oc = channels;
+      });
+      if (pfor_bad.load()) return fail(XIVO_ERR_STATE, "host state machine threw: " + pfor_msg);
+    }
+    {
+      HostScope hu("png_issue");
+      XB_CUDA(png_stage.up(st_copy, stage_bytes));
+      if (int rc = launch_png_decode(st_copy, png_stage.d + table, png_scratch.p, dRing, reinterpret_cast<const PngFrameDesc*>(png_stage.d), B,
+                                     png_status.d))
+        return rc;
+      XB_CUDA(png_status.down(st_copy, B));
+      if (int rc = ring_uploaded(distinct_slots(slot_of))) return rc;
+    }
+    { HostScope hw("wait_png"); if (int rc = wait(st_copy)) return rc; }
+    for (int s = 0; s < B; ++s)
+      if (png_status.h[s] != png::kOk) {
+        ring_next = ring_before;
+        return fail(XIVO_ERR_ARG, "png frame " + std::to_string(s) + ": " + png::status_text(png_status.h[s]));
+      }
     return 0;
   }
 
@@ -1544,6 +1652,23 @@ int xivo_batch_visual_meas(xivo_batch* b, const uint64_t* ts_ns, const uint8_t* 
 int xivo_batch_visual_meas_device(xivo_batch* b, const uint64_t* ts_ns, const uint8_t* const* imgs_dev, int rows, int cols,
                                   int channels, int tracker_only) {
   return visual_meas_impl(b, ts_ns, imgs_dev, rows, cols, channels, tracker_only, true);
+}
+int xivo_batch_visual_meas_png(xivo_batch* b, const uint64_t* ts_ns, const uint8_t* const* png, const size_t* png_bytes, int channels,
+                               int tracker_only) {
+  BATCH_BEGIN;
+  XB_REQUIRE(ts_ns && png && png_bytes, "visual_meas_png: bad arguments");
+  for (int s = 0; s < B_.B; ++s) XB_REQUIRE(png[s], "visual_meas_png: null data");
+  if (channels != 1 && channels != 3) return B_.fail(XIVO_ERR_ARG, "visual_meas_png: channels must be 1 or 3, got " + std::to_string(channels));
+  HostScope ht("visual_meas_png_total");
+  std::vector<int> slot_of(B_.B);
+  if (int rc = B_.decode_png_frames(png, png_bytes, channels, slot_of)) return rc;
+  std::vector<Msg> in(B_.B);
+  for (int s = 0; s < B_.B; ++s) {
+    in[s].ts = ts_ns[s];
+    in[s].type = tracker_only ? 2 : 1;
+    in[s].img_slot = slot_of[s];
+  }
+  return B_.ingest(in);
 }
 int xivo_batch_step(xivo_batch* b, int n_imu, const uint64_t* imu_ts, const double* gyro, const double* accel, const uint64_t* frame_ts,
                     const uint8_t* const* imgs, int rows, int cols, int channels, int on_device) {

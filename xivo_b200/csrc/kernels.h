@@ -56,6 +56,18 @@ int launch_lk_track(cudaStream_t st, const uint8_t* prev_pyr, const uint8_t* nex
                     const int* npts_dev, int max_pts, int batch, int win, int max_iter, double eps, int use_initial_flow,
                     double min_eig);
 
+// ---------------- PNG frames (png_kernels.cu) ----------------
+// one frame of a decode launch: its zlib stream at in + in_off (in_len bytes, the IDAT payloads back to back), its rows x (1 + cols x bpp)
+// bytes of filtered scanlines at scratch + scratch_off, its rows x cols x oc output bytes at out + out_off
+struct PngFrameDesc {
+  unsigned long long in_off, scratch_off, out_off;
+  unsigned long long in_len;
+  int rows, cols;
+  int bpp, channels, bps, oc;  // bytes per pixel, samples per pixel, bytes per sample, output channels
+};
+// png_inflate_kernel + png_unfilter_kernel for n frames; status[i] = png::kOk or the png.cuh status of frame i
+int launch_png_decode(cudaStream_t st, const uint8_t* in, uint8_t* scratch, uint8_t* out, const PngFrameDesc* fr, int n, int* status);
+
 // ---------------- EKF (ekf_kernels.cu) ----------------
 // Error-state layout, /root/reference/src/core.h:40-105 (default build: no online calibration).
 struct EkfLayout {

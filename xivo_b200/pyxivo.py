@@ -118,6 +118,20 @@ class Batch:
         self._keep = imgs
         _check(capi.lib().xivo_batch_visual_meas(self._h, _p(ts), ptrs, rows, cols, ch, int(bool(tracker_only))), "xivo_batch_visual_meas")
 
+    def visual_meas_png(self, ts_ns, blobs, channels=3, tracker_only=False):
+        """visual_meas with the frames given as PNG file bytes (one per sequence, or one shared by all), decoded on the device straight
+        into the frame ring (xivo_batch_visual_meas_png) as cv2.imread decodes them: channels = 3 is IMREAD_COLOR (BGR), channels = 1 is
+        IMREAD_GRAYSCALE of grey / grey + alpha files.  A refused or corrupt file raises XivoError before any sequence's state changes."""
+        if isinstance(blobs, (bytes, bytearray, memoryview)):
+            blobs = [blobs] * self.n
+        blobs = [bytes(x) for x in blobs]
+        if len(blobs) != self.n:
+            raise XivoError(f"expected {self.n} PNG frames (one per sequence), got {len(blobs)}")
+        ts = np.ascontiguousarray(np.broadcast_to(np.asarray(ts_ns, dtype=np.uint64), (self.n,)))
+        src = (C.c_char_p * self.n)(*blobs)
+        sizes = (C.c_size_t * self.n)(*[len(x) for x in blobs])
+        _check(capi.lib().xivo_batch_visual_meas_png(self._h, _p(ts), src, sizes, int(channels), int(bool(tracker_only))), "xivo_batch_visual_meas_png")
+
     def prefetch_frames(self, imgs):
         """Start uploading the frames of the NEXT visual_meas / step call (same arrays) while the current one is computed."""
         imgs, rows, cols, ch = self._check_images(imgs)
@@ -307,13 +321,19 @@ class Estimator:
     def InertialMeas(self, ts, wx, wy, wz, ax, ay, az):
         self._b.inertial_meas(int(ts), [wx, wy, wz], [ax, ay, az])
 
+    def _visual(self, ts, image, tracker_only):
+        if isinstance(image, (str, os.PathLike)):  # cv::imread(path) as the reference's binding does (pybind11/pyxivo.cpp:81-85, :119-123)
+            with open(image, "rb") as f:
+                self._b.visual_meas_png(int(ts), [f.read()], channels=3, tracker_only=tracker_only)
+        else:
+            self._b.visual_meas(int(ts), [image], tracker_only=tracker_only)
+
     def VisualMeas(self, ts, image):
-        if isinstance(image, str):
-            raise XivoError("VisualMeas(path) needs an image decoder; pass the decoded uint8 array instead")
-        self._b.visual_meas(int(ts), [image], tracker_only=False)
+        """image: a decoded uint8 array, or the path of a PNG file (decoded on the device like cv::imread(path))"""
+        self._visual(ts, image, False)
 
     def VisualMeasTrackerOnly(self, ts, image):
-        self._b.visual_meas(int(ts), [image], tracker_only=True)
+        self._visual(ts, image, True)
 
     def VisualMeasPointCloud(self, ts, feature_ids, xp_and_depths):
         self._b.visual_meas_pointcloud(int(ts), [np.asarray(feature_ids)], [np.asarray(xp_and_depths)], tracker_only=False)
