@@ -24,12 +24,13 @@ struct DevBuf {
     p = nullptr;
     n = 0;
   }
-  void alloc(size_t count) {
+  // releases what it held; on failure the buffer is left empty
+  bool alloc(size_t count) {
     release();
-    n = count;
-    if (count == 0) return;
-    failed = cudaMalloc(reinterpret_cast<void**>(&p), count * sizeof(T)) != cudaSuccess;
+    failed = count && cudaMalloc(reinterpret_cast<void**>(&p), count * sizeof(T)) != cudaSuccess;
     if (failed) p = nullptr;
+    else n = count;
+    return !failed;
   }
   bool ok() const { return !failed; }
 };

@@ -48,63 +48,103 @@ extern std::atomic<unsigned long long> g_launches;
 // Default: the copy engine (with the tables of every phase fetched by kernels, DMA frames delay them least).
 static std::atomic<int> g_frame_ingest{(getenv("XIVO_ZEROCOPY") && getenv("XIVO_ZEROCOPY")[0] == '1') ? 0 : 1};
 
-// Pinned host mirror + device array.
+// A host table and its device copy, n elements each.  A View does not own them: its tables live inside a Mirror blob (one upload /
+// download of the blob then covers several tables).
 template <typename T>
-struct Mirror {
+struct View {
   T* h = nullptr;
   T* d = nullptr;
   size_t n = 0;
-  // zero_copy: a host-written table that one kernel reads once.  The kernel reads the pinned host memory in place (mapped into the
-  // device address space), so there is no cudaMemcpyAsync call and — what matters end to end — the table does not queue behind the
-  // frame uploads in the H2D copy engine's FIFO.  The host must not rewrite it before the consuming kernel has finished (every table
-  // is rewritten only after the wait that ends its phase).
-  bool zero_copy = false;
-  T* hd = nullptr;  // device alias of the pinned host copy (alloc_fetchable): what fetch_kernel reads
-  // pinned + mapped host copy and a device copy: the upload is a kernel that reads the host copy over PCIe (Batch::up_blob)
-  bool alloc_fetchable(size_t count) {
-    n = count;
-    if (!count) return true;
-    if (cudaHostAlloc(reinterpret_cast<void**>(&h), count * sizeof(T), cudaHostAllocMapped) != cudaSuccess) return false;
-    memset(h, 0, count * sizeof(T));
-    if (cudaHostGetDevicePointer(reinterpret_cast<void**>(&hd), h, 0) != cudaSuccess) return false;
-    if (cudaMalloc(reinterpret_cast<void**>(&d), count * sizeof(T)) != cudaSuccess) return false;
-    return cudaMemset(d, 0, count * sizeof(T)) == cudaSuccess;
-  }
-  bool alloc(size_t count, bool zc = false) {
-    n = count;
-    zero_copy = zc;
-    if (!count) return true;
-    if (zc) {
-      if (cudaHostAlloc(reinterpret_cast<void**>(&h), count * sizeof(T), cudaHostAllocMapped) != cudaSuccess) return false;
-      memset(h, 0, count * sizeof(T));
-      return cudaHostGetDevicePointer(reinterpret_cast<void**>(&d), h, 0) == cudaSuccess;
-    }
-    if (cudaMallocHost(reinterpret_cast<void**>(&h), count * sizeof(T)) != cudaSuccess) return false;
-    if (cudaMalloc(reinterpret_cast<void**>(&d), count * sizeof(T)) != cudaSuccess) return false;
-    memset(h, 0, count * sizeof(T));
-    return cudaMemset(d, 0, count * sizeof(T)) == cudaSuccess;
-  }
-  // storage carved out of a parent blob (one upload / download of the parent then covers several tables)
-  bool borrowed = false;
-  void adopt(void* h_, void* d_, size_t count) {
-    h = static_cast<T*>(h_); d = static_cast<T*>(d_); n = count; borrowed = true;
-  }
-  void release() {
-    if (!borrowed) {
-      if (h) cudaFreeHost(h);
-      if (d && !zero_copy) cudaFree(d);
-    }
-    h = d = nullptr;
-  }
   cudaError_t up(cudaStream_t st, size_t count = 0, size_t off = 0) {
-    Prof::get().h2d += (count ? count : n) * sizeof(T);  // the bytes cross PCIe either way
-    if (zero_copy) return cudaSuccess;
+    Prof::get().h2d += (count ? count : n) * sizeof(T);
     return cudaMemcpyAsync(d + off, h + off, (count ? count : n) * sizeof(T), cudaMemcpyHostToDevice, st);
   }
   cudaError_t down(cudaStream_t st, size_t count = 0, size_t off = 0) {
     Prof::get().d2h += (count ? count : n) * sizeof(T);
     return cudaMemcpyAsync(h + off, d + off, (count ? count : n) * sizeof(T), cudaMemcpyDeviceToHost, st);
   }
+};
+
+// Pinned host mirror + device array, both zeroed, owned.  fetchable: the host copy is also mapped into the device address space (hd),
+// so that its upload can be a kernel that reads it over PCIe (Batch::up_blob).
+template <typename T>
+struct Mirror : View<T> {
+  using View<T>::h;
+  using View<T>::d;
+  using View<T>::n;
+  T* hd = nullptr;
+  Mirror() = default;
+  Mirror(const Mirror&) = delete;
+  Mirror& operator=(const Mirror&) = delete;
+  ~Mirror() { release(); }
+  void release() {
+    if (h) cudaFreeHost(h);
+    if (d) cudaFree(d);
+    h = d = hd = nullptr;
+    n = 0;
+  }
+  // releases what it held; on failure the mirror is left empty
+  bool alloc(size_t count, bool fetchable = false) {
+    release();
+    if (!count) return true;
+    const size_t bytes = count * sizeof(T);
+    if (cudaHostAlloc(reinterpret_cast<void**>(&h), bytes, fetchable ? cudaHostAllocMapped : cudaHostAllocDefault) != cudaSuccess) {
+      h = nullptr;
+      return false;
+    }
+    memset(h, 0, bytes);
+    if ((fetchable && cudaHostGetDevicePointer(reinterpret_cast<void**>(&hd), h, 0) != cudaSuccess) ||
+        cudaMalloc(reinterpret_cast<void**>(&d), bytes) != cudaSuccess)
+      d = nullptr;
+    if (!d || cudaMemset(d, 0, bytes) != cudaSuccess) {
+      release();
+      return false;
+    }
+    n = count;
+    return true;
+  }
+};
+
+// Several tables back to back in one fetchable Mirror blob, each padded to a multiple of `pad` bytes, the blob to 16-byte units
+// (fetch_kernel's loads).  put() returns a table's offset; with a base (h, d) it also points the table's view there.
+struct BlobLayout {
+  size_t pad, off = 0;
+  unsigned char *h = nullptr, *d = nullptr;
+  template <typename T>
+  size_t put(View<T>& v, size_t count) {
+    const size_t o = off;
+    off += (count * sizeof(T) + pad - 1) / pad * pad;
+    if (h) { v.h = reinterpret_cast<T*>(h + o); v.d = reinterpret_cast<T*>(d + o); v.n = count; }
+    return o;
+  }
+};
+// Allocates blob b for the tables that tables(BlobLayout&) puts, in that order, and binds their views.
+template <typename Tables>
+static bool carve(Mirror<unsigned char>& b, Tables tables, size_t pad = 16) {
+  BlobLayout size{pad};
+  tables(size);
+  if (!b.alloc((size.off + 15) & ~(size_t)15, true)) return false;
+  BlobLayout bind{pad, 0, b.h, b.d};
+  tables(bind);
+  return true;
+}
+
+// Owners of a non-blocking stream and of a timing-free event.
+struct Stream {
+  cudaStream_t s = nullptr;
+  Stream() { cudaStreamCreateWithFlags(&s, cudaStreamNonBlocking); }
+  Stream(const Stream&) = delete;
+  Stream& operator=(const Stream&) = delete;
+  ~Stream() { if (s) cudaStreamDestroy(s); }
+  operator cudaStream_t() const { return s; }
+};
+struct Event {
+  cudaEvent_t e = nullptr;
+  Event() { cudaEventCreateWithFlags(&e, cudaEventDisableTiming); }
+  Event(const Event&) = delete;
+  Event& operator=(const Event&) = delete;
+  ~Event() { if (e) cudaEventDestroy(e); }
+  operator cudaEvent_t() const { return e; }
 };
 
 // Completion of a stream without CUDA calls in the wait loop: the driver thread asks the stream to write a ticket number into mapped
@@ -152,12 +192,18 @@ struct StreamTicket {
   unsigned* h = nullptr;  // mapped pinned word the stream writes
   unsigned* d = nullptr;  // its device address
   unsigned next = 0;      // last ticket handed out
+  StreamTicket() = default;
+  StreamTicket(const StreamTicket&) = delete;
+  StreamTicket& operator=(const StreamTicket&) = delete;
+  ~StreamTicket() { if (h) cudaFreeHost(h); }
   bool alloc() {
-    if (cudaHostAlloc(reinterpret_cast<void**>(&h), 64, cudaHostAllocMapped) != cudaSuccess) return false;
+    if (cudaHostAlloc(reinterpret_cast<void**>(&h), 64, cudaHostAllocMapped) != cudaSuccess) {
+      h = nullptr;
+      return false;
+    }
     memset(h, 0, 64);
     return cudaHostGetDevicePointer(reinterpret_cast<void**>(&d), h, 0) == cudaSuccess;
   }
-  void release() { if (h) cudaFreeHost(h); h = d = nullptr; }
   bool reached(unsigned t) const { return (int)(*reinterpret_cast<volatile unsigned*>(h) - t) >= 0; }
 };
 
@@ -194,29 +240,29 @@ class Batch {
   int B, N, maxops, max_sub;
   int cov_tc = 0;  // covariance downdate on the tensor cores ("covariance_update": "tf32x3")
   bool use_1pt = false;       // filter-level 1-point RANSAC: the gate phase also returns diag(P), two extra device phases on demand
-  double* dP0 = nullptr;      // P_ backup of OnePointRANSAC (BackupState / RestoreState), allocated at the first use
+  DevBuf<double> dP0;         // P_ backup of OnePointRANSAC (BackupState / RestoreState), allocated at the first use
   std::vector<std::vector<Feature*>> table_order;  // per sequence: index space of the device feature table of this frame
   TcOperands tcops;  // its TF32 operand buffers + tensor maps (ekf_cov_tc2_kernel); XIVO_TC_V1=1 keeps the first formulation
-  uint32_t *dKt32 = nullptr, *dHP32 = nullptr;
+  DevBuf<uint32_t> dKt32, dHP32;
   EkfLayout lay;
   std::vector<std::unique_ptr<Estimator>> est;
   // EKF device state
-  double* dP = nullptr;
-  double *dHP = nullptr, *dKt = nullptr, *dErr = nullptr;
-  FeatJac* dJac = nullptr;
+  DevBuf<double> dP, dHP, dKt, dErr;
+  DevBuf<FeatJac> dJac;
   Mirror<CameraParams> cam;
-  Mirror<double> X, groups, fx, fxp, R, mh, pack;
-  Mirror<int> fref, fsind, nfeat, sel, nsel;
+  Mirror<double> R, mh, pack;
+  View<double> X, groups, fx, fxp;
+  View<int> fref, fsind, nfeat, sel, nsel;
   // Host-written tables go down as ONE copy per phase: each phase owns a pinned + device blob, its tables are views into it, and the
   // variable-length table (sub-filter inputs, packed edit list, packed stage records) sits last so that only its used part is copied.
   Mirror<unsigned char> blobS, blobJ, blobU, blobI[2];
   size_t blobS_fixed = 0, blobJ_fixed = 0, blobU_fixed = 0, blobI_fixed = 0;  // bytes in front of the variable-length table
-  Mirror<EditOp> opsJ, opsU;              // packed edit lists: filter b owns [first[b], first[b] + nops[b])
-  Mirror<int> nopsJ, firstJ, nopsU, firstU;
-  Mirror<SubfilterIn> sub_in;
+  View<EditOp> opsJ, opsU;              // packed edit lists: filter b owns [first[b], first[b] + nops[b])
+  View<int> nopsJ, firstJ, nopsU, firstU;
+  View<SubfilterIn> sub_in;
   Mirror<SubfilterOut> sub_out;
-  Mirror<ImuStep> stg[2];  // packed Runge-Kutta sub-step records of all filters, two staging halves used alternately
-  Mirror<int> stg_first[2], stg_n[2];
+  View<ImuStep> stg[2];  // packed Runge-Kutta sub-step records of all filters, two staging halves used alternately
+  View<int> stg_first[2], stg_n[2];
   int stg_half = 0;
   unsigned stg_busy[2] = {0, 0};  // st2 ticket after which the half may be refilled (0 = free)
   Mirror<ImuConst> icst;
@@ -227,17 +273,17 @@ class Batch {
   StreamTicket tk1, tk2, tkc;  // completion flags of st1 / st2 / st_copy
   // The covariance side (IMU propagation, slot edits, Jacobians, update) runs on its own stream so that it
   // overlaps the image tracker's kernels and host phases, which use ctx->stream.
-  cudaStream_t st2 = nullptr;
+  Stream st2;
   // Frames are uploaded on their own stream: the message heap releases a frame several messages after it was
   // pushed, so its copy overlaps the tracking of the frame released now.  ring_ev[slot] orders the two.
-  cudaStream_t st_copy = nullptr;
-  std::vector<cudaEvent_t> ring_ev;
+  Stream st_copy;
+  std::vector<Event> ring_ev;
   // tracker device state (allocated at the first image)
   bool img_ready = false;
   int rows = 0, cols = 0, cn = 0, ring_n = 0, max_pts = 0, max_kp = 0;
   PyrDesc pd;
-  uint8_t* dRing = nullptr;   // B x ring_n x img_bytes
-  uint8_t* dPyr = nullptr;    // B x 2 x pd.total
+  DevBuf<uint8_t> dRing;  // B x ring_n x img_bytes
+  DevBuf<uint8_t> dPyr;   // B x 2 x pd.total
   std::vector<int> ring_next, prev_slot;
   // xivo_batch_visual_meas_png: pinned staging [frame table | IDAT payloads] + its device copy, the decoder's scratch of filtered scanlines
   // and the per-frame status words; all grown on demand to what a call needs
@@ -247,13 +293,15 @@ class Batch {
   // xivo_batch_prefetch_frames: host pointers and ring slots of the frames whose upload is already in flight on st_copy
   struct Prefetched { std::vector<const uint8_t*> ptr; std::vector<int> slot; };
   std::deque<Prefetched> pref;  // oldest first; at most two (the frame about to be consumed and the one after it)
-  Mirror<unsigned long long> off_prev, off_cur;
-  Mirror<const uint8_t*> frame_ptr, ingest_ptr;  // ring slot of the frame being tracked; sources of a device-resident ingest
-  Mirror<unsigned long long> ingest_off;
-  Mirror<unsigned char> blobG;                   // [ingest_ptr | ingest_off]: one copy per gather launch
-  Mirror<float> pts0, pts1, lkerr;
+  View<unsigned long long> off_prev, off_cur;
+  View<const uint8_t*> frame_ptr, ingest_ptr;  // ring slot of the frame being tracked; sources of a device-resident ingest
+  View<unsigned long long> ingest_off;
+  Mirror<unsigned char> blobG;                 // [ingest_ptr | ingest_off]: one copy per gather launch
+  View<float> pts0, pts1;
+  Mirror<float> lkerr;
   Mirror<uint8_t> lkst;
-  Mirror<int> npts, kpcount;
+  View<int> npts;
+  Mirror<int> kpcount;
   Mirror<unsigned> kp;
   // TMA pyramid passes (pyrdown_tma_kernel): tensor maps over the frame ring (level-0 source) and over the pyramid levels
   bool tma_pyr = false;
@@ -262,13 +310,13 @@ class Batch {
   bool tm_lvl_ok[kMaxPyrLevels] = {false};
   bool tma_fast = false;  // FAST tiles by TMA (fast_pair_tma_kernel): tensor map over the level-0 images of the pyramid buffer
   CUtensorMap tm_fast;
-  Mirror<int> ring_img, pyr_img;  // per sequence: image index of the new frame inside the ring map / of the current pyramid inside the level maps
+  View<int> ring_img, pyr_img;  // per sequence: image index of the new frame inside the ring map / of the current pyramid inside the level maps
   // device-side tracker decisions (track_accept_kernel / track_select_kernel)
   bool dev_decide = false;
-  Mirror<int> tkind, tneed, tnnew;
-  Mirror<uint8_t> tstat;
-  Mirror<unsigned> tnewkp;
-  Mirror<unsigned long long> fast_off;  // FAST selector: pyramid offset of the sequences that may need a detection
+  View<int> tkind, tneed, tnnew;
+  View<uint8_t> tstat;
+  View<unsigned> tnewkp;
+  View<unsigned long long> fast_off;  // FAST selector: pyramid offset of the sequences that may need a detection
   // descriptor path (tracker.cpp:231-292, :341-460, :530-565): BRIEF-32 at the tracked positions and at the detected keypoints, Hamming
   // nearest neighbours for the cross-checked matcher.  Allocated when the tracker extracts descriptors; decisions then stay on the host.
   bool desc_on = false;
@@ -284,8 +332,6 @@ class Batch {
   Batch(xivo_ctx* c, const Json& cfg, int nseq, EkfLayout l, bool tracker_only) : ctx(c), B(nseq), lay(l), cfg0(cfg) {
     N = lay.N();
     st1 = ctx->stream;
-    cudaStreamCreateWithFlags(&st2, cudaStreamNonBlocking);
-    cudaStreamCreateWithFlags(&st_copy, cudaStreamNonBlocking);
     for (int b = 0; b < B; ++b) {
       est.emplace_back(new Estimator(cfg, lay, tracker_only));
       est.back()->compact_records = true;  // imu_cov_propagate rebuilds the intermediate Runge-Kutta stages itself
@@ -295,72 +341,33 @@ class Batch {
     table_order.resize(B);
     maxops = 4 * (lay.F + lay.G) + 16;
     max_sub = est[0]->tc.num_features_max + 8;
-    bool ok = cudaMalloc(reinterpret_cast<void**>(&dP), sizeof(double) * B * N * N) == cudaSuccess &&
-              cudaMalloc(reinterpret_cast<void**>(&dHP), sizeof(double) * B * 2 * lay.F * N) == cudaSuccess &&
-              cudaMalloc(reinterpret_cast<void**>(&dKt), sizeof(double) * B * 2 * lay.F * N) == cudaSuccess &&
-              cudaMalloc(reinterpret_cast<void**>(&dErr), sizeof(double) * B * N) == cudaSuccess &&
-              cudaMalloc(reinterpret_cast<void**>(&dJac), sizeof(FeatJac) * B * lay.F) == cudaSuccess;
-    ok = ok && cam.alloc(B) && R.alloc(B) && mh.alloc((size_t)B * lay.F + (size_t)B * N) && pack.alloc((size_t)B * (2 * N + 529)) && sub_out.alloc((size_t)B * max_sub) &&
-         icst.alloc(B) && pmm0.alloc((size_t)B * 529) && tk1.alloc() && tk2.alloc() && tkc.alloc();
-    if (ok) {  // the per-phase upload blobs and the table views inside them
-      struct Carve {
-        size_t off = 0;
-        size_t take(size_t bytes) { const size_t o = off; off += (bytes + 15) & ~(size_t)15; return o; }
-      };
-      const size_t nB = (size_t)B, nF = (size_t)B * lay.F;
-      {  // sub-filter phase: [X | sub_in ...]
-        Carve c;
-        const size_t oX = c.take(nB * kPoseDoubles * 8);
-        blobS_fixed = c.off;
-        const size_t oS = c.take(nB * max_sub * sizeof(SubfilterIn));
-        ok = ok && blobS.alloc_fetchable((c.off + 15) & ~(size_t)15);
-        if (ok) { X.adopt(blobS.h + oX, blobS.d + oX, nB * kPoseDoubles); sub_in.adopt(blobS.h + oS, blobS.d + oS, nB * max_sub); }
-      }
-      {  // Jacobian / gate phase: [nfeat | nops | first | fref | fsind | fxp | fx | groups | ops ...]
-        Carve c;
-        const size_t o0 = c.take(nB * 4), o1 = c.take(nB * 4), o2 = c.take(nB * 4), o3 = c.take(nF * 4), o4 = c.take(nF * 4), o5 = c.take(nF * 2 * 8),
-                     o6 = c.take(nF * 3 * 8), o7 = c.take(nB * lay.G * kGroupDoubles * 8);
-        blobJ_fixed = c.off;
-        const size_t o8 = c.take(nB * maxops * sizeof(EditOp));
-        ok = ok && blobJ.alloc_fetchable((c.off + 15) & ~(size_t)15);
-        if (ok) {
-          auto H = [&](size_t o) { return (void*)(blobJ.h + o); };
-          auto D = [&](size_t o) { return (void*)(blobJ.d + o); };
-          nfeat.adopt(H(o0), D(o0), nB); nopsJ.adopt(H(o1), D(o1), nB); firstJ.adopt(H(o2), D(o2), nB); fref.adopt(H(o3), D(o3), nF);
-          fsind.adopt(H(o4), D(o4), nF); fxp.adopt(H(o5), D(o5), nF * 2); fx.adopt(H(o6), D(o6), nF * 3);
-          groups.adopt(H(o7), D(o7), nB * lay.G * kGroupDoubles); opsJ.adopt(H(o8), D(o8), nB * maxops);
-        }
-      }
-      {  // update phase: [nsel | nops | first | sel | ops ...]
-        Carve c;
-        const size_t o0 = c.take(nB * 4), o1 = c.take(nB * 4), o2 = c.take(nB * 4), o3 = c.take(nF * 4);
-        blobU_fixed = c.off;
-        const size_t o4 = c.take(nB * maxops * sizeof(EditOp));
-        ok = ok && blobU.alloc_fetchable((c.off + 15) & ~(size_t)15);
-        if (ok) {
-          auto H = [&](size_t o) { return (void*)(blobU.h + o); };
-          auto D = [&](size_t o) { return (void*)(blobU.d + o); };
-          nsel.adopt(H(o0), D(o0), nB); nopsU.adopt(H(o1), D(o1), nB); firstU.adopt(H(o2), D(o2), nB); sel.adopt(H(o3), D(o3), nF);
-          opsU.adopt(H(o4), D(o4), nB * maxops);
-        }
-      }
-      for (int h = 0; h < 2 && ok; ++h) {  // IMU sub-step records: [first | n | steps ...], two staging halves
-        Carve c;
-        const size_t o0 = c.take(nB * 4), o1 = c.take(nB * 4);
-        blobI_fixed = c.off;
-        const size_t o2 = c.take(nB * kMaxSteps * sizeof(ImuStep));
-        ok = ok && blobI[h].alloc_fetchable((c.off + 15) & ~(size_t)15);
-        if (ok) {
-          stg_first[h].adopt(blobI[h].h + o0, blobI[h].d + o0, nB); stg_n[h].adopt(blobI[h].h + o1, blobI[h].d + o1, nB);
-          stg[h].adopt(blobI[h].h + o2, blobI[h].d + o2, nB * kMaxSteps);
-        }
-      }
-    }
+    const size_t nB = (size_t)B, nF = (size_t)B * lay.F;
+    bool ok = dP.alloc(nB * N * N) && dHP.alloc(nF * 2 * N) && dKt.alloc(nF * 2 * N) && dErr.alloc(nB * N) && dJac.alloc(nF);
+    ok = ok && cam.alloc(B) && R.alloc(B) && mh.alloc(nF + nB * N) && pack.alloc(nB * (2 * N + 529)) && sub_out.alloc(nB * max_sub) &&
+         icst.alloc(B) && pmm0.alloc(nB * 529) && tk1.alloc() && tk2.alloc() && tkc.alloc();
+    // the per-phase upload blobs and the table views inside them; the variable-length table last
+    ok = ok && carve(blobS, [&](BlobLayout& t) {  // sub-filter phase
+           t.put(X, nB * kPoseDoubles);
+           blobS_fixed = t.put(sub_in, nB * max_sub);
+         });
+    ok = ok && carve(blobJ, [&](BlobLayout& t) {  // Jacobian / gate phase
+           t.put(nfeat, nB); t.put(nopsJ, nB); t.put(firstJ, nB); t.put(fref, nF); t.put(fsind, nF); t.put(fxp, nF * 2); t.put(fx, nF * 3);
+           t.put(groups, nB * lay.G * kGroupDoubles);
+           blobJ_fixed = t.put(opsJ, nB * maxops);
+         });
+    ok = ok && carve(blobU, [&](BlobLayout& t) {  // update phase
+           t.put(nsel, nB); t.put(nopsU, nB); t.put(firstU, nB); t.put(sel, nF);
+           blobU_fixed = t.put(opsU, nB * maxops);
+         });
+    for (int h = 0; h < 2; ++h)  // IMU sub-step records, two staging halves
+      ok = ok && carve(blobI[h], [&](BlobLayout& t) {
+             t.put(stg_first[h], nB); t.put(stg_n[h], nB);
+             blobI_fixed = t.put(stg[h], nB * kMaxSteps);
+           });
     if (ok && cov_tc && !(getenv("XIVO_TC_V1") && getenv("XIVO_TC_V1")[0] == '1')) {
       const size_t words = tc_operand_words(N, 2 * lay.F, B);
-      ok = cudaMalloc(reinterpret_cast<void**>(&dKt32), words * 4) == cudaSuccess && cudaMalloc(reinterpret_cast<void**>(&dHP32), words * 4) == cudaSuccess &&
-           cudaMemset(dKt32, 0, words * 4) == cudaSuccess && cudaMemset(dHP32, 0, words * 4) == cudaSuccess &&
-           tc_operands_init(&tcops, N, 2 * lay.F, B, dKt32, dHP32) == 0;
+      ok = dKt32.alloc(words) && dHP32.alloc(words) && cudaMemset(dKt32.p, 0, words * 4) == cudaSuccess && cudaMemset(dHP32.p, 0, words * 4) == cudaSuccess &&
+           tc_operands_init(&tcops, N, 2 * lay.F, B, dKt32.p, dHP32.p) == 0;
     }
     if (!ok) throw std::runtime_error(std::string("device allocation failed: ") + cudaGetErrorString(cudaGetLastError()));
     for (int b = 0; b < B; ++b) set_filter_tables(b);
@@ -368,7 +375,7 @@ class Batch {
     R.up(st1);
     icst.up(st1);
     pmm0.up(st1);
-    if (launch_cov_init(st1, N, dP, pmm0.d, 0, B)) throw std::runtime_error(std::string("initial covariance: ") + cudaGetErrorString(cudaGetLastError()));
+    if (launch_cov_init(st1, N, dP.p, pmm0.d, 0, B)) throw std::runtime_error(std::string("initial covariance: ") + cudaGetErrorString(cudaGetLastError()));
     cudaStreamSynchronize(st1);
   }
   // Host mirrors of sequence b's per-filter device tables (camera, measurement noise, IMU constants, initial motion covariance) from
@@ -428,26 +435,16 @@ class Batch {
     XB_CUDA(R.up(st2, 1, seq));
     XB_CUDA(icst.up(st2, 1, seq));
     XB_CUDA(pmm0.up(st2, 529, (size_t)seq * 529));
-    if (int rc = launch_cov_init(st2, N, dP, pmm0.d, seq, 1)) return rc;
+    if (int rc = launch_cov_init(st2, N, dP.p, pmm0.d, seq, 1)) return rc;
     g_launches += 1;
     reset_busy = tk2.next + 1;  // the next ticket of st2 lies behind these uploads
     return 0;
   }
+  // the members free themselves once no queued work can touch them any more
   ~Batch() {
     cudaStreamSynchronize(st1);
-    if (st2) { cudaStreamSynchronize(st2); cudaStreamDestroy(st2); }
-    if (st_copy) { cudaStreamSynchronize(st_copy); cudaStreamDestroy(st_copy); }
-    for (cudaEvent_t e : ring_ev) cudaEventDestroy(e);
-    for (void* p : {(void*)dP, (void*)dHP, (void*)dKt, (void*)dErr, (void*)dJac, (void*)dRing, (void*)dPyr, (void*)dKt32, (void*)dHP32, (void*)dP0})
-      if (p) cudaFree(p);
-    cam.release(); R.release(); mh.release(); pack.release(); sub_out.release(); blobS.release(); blobJ.release(); blobU.release();
-    blobI[0].release(); blobI[1].release(); tk1.release(); tk2.release(); tkc.release();
-    png_stage.release(); png_status.release(); png_scratch.release();
-    icst.release(); pmm0.release(); blobG.release();
-    lkerr.release(); lkst.release(); kpcount.release();
-    kp.release(); tt.release();
-    descT.release(); validT.release(); kpxy.release(); nkps.release(); nq.release(); descK.release(); validK.release(); qdesc.release();
-    bestT_idx.release(); bestT_dist.release(); bestQ_idx.release(); bestQ_dist.release();
+    cudaStreamSynchronize(st2);
+    cudaStreamSynchronize(st_copy);
   }
 
   int fail(int code, const std::string& m) {
@@ -458,7 +455,7 @@ class Batch {
   // ---- staging helpers -------------------------------------------------------------------
   cudaError_t up_blob(Mirror<unsigned char>& b, size_t bytes, cudaStream_t st) {
     Prof::get().h2d += bytes;
-    if (!b.hd || !bytes) return bytes ? cudaMemcpyAsync(b.d, b.h, bytes, cudaMemcpyHostToDevice, st) : cudaSuccess;
+    if (!bytes) return cudaSuccess;
     const unsigned n16 = (unsigned)((bytes + 15) / 16);  // blobs are allocated in 16-byte units
     const unsigned ctas = std::max(1u, std::min(64u, (n16 + 1023) / 1024));
     fetch_kernel<<<ctas, 256, 0, st>>>(reinterpret_cast<const uint4*>(b.hd), reinterpret_cast<uint4*>(b.d), n16);
@@ -466,7 +463,7 @@ class Batch {
     return cudaGetLastError();
   }
   // pack the pending covariance edits of the given sequences into ops (filter b: [first[b], first[b] + nops[b])); *total = entries used
-  int stage_edits(const std::vector<int>& act, Mirror<EditOp>& ops, Mirror<int>& first, Mirror<int>& nops, int* total) {
+  int stage_edits(const std::vector<int>& act, View<EditOp>& ops, View<int>& first, View<int>& nops, int* total) {
     for (int b = 0; b < B; ++b) { nops.h[b] = 0; first.h[b] = 0; }
     int n = 0;
     for (int b : act) {
@@ -523,7 +520,7 @@ class Batch {
         more = more || cur[b] < est[b]->steps.size();
       }
       XB_CUDA(up_blob(blobI[h], blobI_fixed + (size_t)total * sizeof(ImuStep), st));
-      if (int rc = launch_imu_cov_propagate(st, N, dP, stg[h].d, stg_first[h].d, stg_n[h].d, icst.d, B)) return rc;
+      if (int rc = launch_imu_cov_propagate(st, N, dP.p, stg[h].d, stg_first[h].d, stg_n[h].d, icst.d, B)) return rc;
       stg_busy[h] = tk2.next + 1;  // the next ticket of st2 lies behind this launch
       stg_half ^= 1;
       g_launches += 1;
@@ -548,7 +545,7 @@ class Batch {
     int nops_total = 0;
     if (int rc = stage_edits(act, opsJ, firstJ, nopsJ, &nops_total)) return rc;
     XB_CUDA(up_blob(blobJ, blobJ_fixed + (size_t)nops_total * sizeof(EditOp), st));
-    if (int rc = launch_cov_edit(st, N, dP, opsJ.d, nopsJ.d, maxops, B, firstJ.d)) return rc;
+    if (int rc = launch_cov_edit(st, N, dP.p, opsJ.d, nopsJ.d, maxops, B, firstJ.d)) return rc;
     g_launches += 1;
     { HostScope hw("wait_flush"); if (int rc = wait(st)) return rc; }
     return 0;
@@ -675,7 +672,7 @@ class Batch {
       XB_CUDA(up_blob(blobG, blobG.n, st_copy));  // [sources | ring offsets]
       // host sources: one warp per frame with four loads in flight still fills the link when several batches pull at once, and hogs it
       // less for the other batches' table fetches than wider grids do
-      if (int rc = launch_gather_frames(st_copy, ingest_ptr.d, dRing, 0, ingest_off.d, ib, B, on_device ? 64 : 1, on_device ? 256 : 32)) return rc;
+      if (int rc = launch_gather_frames(st_copy, ingest_ptr.d, dRing.p, 0, ingest_off.d, ib, B, on_device ? 64 : 1, on_device ? 256 : 32)) return rc;
       g_launches += 1;
     } else {
       // copy engine: runs of sequences whose sources are evenly spaced (frames of one pinned pool) and whose ring slots agree go down as
@@ -688,12 +685,12 @@ class Batch {
           if (stride >= ib) {
             while (e + 1 < B && slot_of[e + 1] == slot_of[s] && imgs[e + 1] > imgs[e] && (size_t)(imgs[e + 1] - imgs[e]) == stride) ++e;
             ++e;
-            XB_CUDA(cudaMemcpy2DAsync(dRing + ingest_off.h[s], (size_t)ring_n * ib, imgs[s], stride, ib, (size_t)(e - s), cudaMemcpyHostToDevice, st_copy));
+            XB_CUDA(cudaMemcpy2DAsync(dRing.p + ingest_off.h[s], (size_t)ring_n * ib, imgs[s], stride, ib, (size_t)(e - s), cudaMemcpyHostToDevice, st_copy));
             s = e;
             continue;
           }
         }
-        XB_CUDA(cudaMemcpyAsync(dRing + ingest_off.h[s], imgs[s], ib, cudaMemcpyHostToDevice, st_copy));
+        XB_CUDA(cudaMemcpyAsync(dRing.p + ingest_off.h[s], imgs[s], ib, cudaMemcpyHostToDevice, st_copy));
         ++s;
       }
     }
@@ -760,14 +757,9 @@ class Batch {
       scratch += (size_t)info[s].raw_bytes();
     }
     const size_t stage_bytes = table + zsum;
-    if (png_stage.n < stage_bytes) {  // grown to 1.25 x the need: frames of one sequence compress to similar sizes
-      png_stage.release();
-      if (!png_stage.alloc(stage_bytes + stage_bytes / 4)) return fail(XIVO_ERR_CUDA, "png staging allocation failed");
-    }
-    if (png_scratch.n < scratch) {
-      png_scratch.alloc(scratch + scratch / 4);
-      if (!png_scratch.ok()) return fail(XIVO_ERR_CUDA, "png scratch allocation failed");
-    }
+    // grown to 1.25 x the need: frames of one sequence compress to similar sizes
+    if (png_stage.n < stage_bytes && !png_stage.alloc(stage_bytes + stage_bytes / 4)) return fail(XIVO_ERR_CUDA, "png staging allocation failed");
+    if (png_scratch.n < scratch && !png_scratch.alloc(scratch + scratch / 4)) return fail(XIVO_ERR_CUDA, "png scratch allocation failed");
     if (png_status.n < (size_t)B && !png_status.alloc(B)) return fail(XIVO_ERR_CUDA, "png status allocation failed");
     // pending prefetches are dropped as for any call with other buffers; ring_next after that is what a refusal restores
     if (!pref.empty()) {
@@ -804,7 +796,7 @@ class Batch {
     {
       HostScope hu("png_issue");
       XB_CUDA(png_stage.up(st_copy, stage_bytes));
-      if (int rc = launch_png_decode(st_copy, png_stage.d + table, png_scratch.p, dRing, reinterpret_cast<const PngFrameDesc*>(png_stage.d), B,
+      if (int rc = launch_png_decode(st_copy, png_stage.d + table, png_scratch.p, dRing.p, reinterpret_cast<const PngFrameDesc*>(png_stage.d), B,
                                      png_status.d))
         return rc;
       XB_CUDA(png_status.down(st_copy, B));
@@ -835,10 +827,11 @@ class Batch {
     max_pts = e0.tc.num_features_max + 8;
     max_kp = std::max(4096, std::min(1 << 16, rows * cols / 8));
     const size_t ib = (size_t)rows * cols * cn;
-    bool ok = cudaMalloc(reinterpret_cast<void**>(&dRing), (size_t)B * ring_n * ib) == cudaSuccess &&
-              cudaMalloc(reinterpret_cast<void**>(&dPyr), (size_t)B * 2 * pd.total) == cudaSuccess;
-    ok = ok && blobG.alloc_fetchable((size_t)B * 16) && lkerr.alloc((size_t)B * max_pts) && lkst.alloc((size_t)B * max_pts) && kpcount.alloc(B) &&
-         kp.alloc((size_t)B * max_kp);
+    const size_t nB = (size_t)B, npt = (size_t)B * max_pts, nk = (size_t)B * max_kp;
+    bool ok = dRing.alloc(nB * ring_n * ib) && dPyr.alloc(nB * 2 * pd.total);
+    // [sources | ring offsets], 8-byte entries back to back
+    ok = ok && carve(blobG, [&](BlobLayout& t) { t.put(ingest_ptr, nB); t.put(ingest_off, nB); }, 8);
+    ok = ok && lkerr.alloc(npt) && lkst.alloc(npt) && kpcount.alloc(B) && kp.alloc(nk);
     // the accept / select decisions run on the device unless the homography stage (host code between the two) is on, the mask does
     // not fit into shared memory, or XIVO_HOST_TRACKER_DECISIONS=1 asks for the host path (parity tests compare the two)
     {
@@ -846,55 +839,36 @@ class Batch {
       dev_decide = !e0.tc.do_outlier_rejection && !e0.tc.extract_descriptor && track_mask_bytes(rows, cols) <= 200 * 1024 && max_pts <= 1024 && !(hd && hd[0] == '1');
     }
     desc_on = e0.tc.extract_descriptor;
-    if (ok && desc_on) {
-      const size_t npt = (size_t)B * max_pts, nk = (size_t)B * max_kp;
+    if (ok && desc_on)
       ok = descT.alloc(npt * 32) && validT.alloc(npt) && kpxy.alloc(nk * 2) && nkps.alloc(B) && nq.alloc(B) && descK.alloc(nk * 32) && validK.alloc(nk) &&
            qdesc.alloc(npt * 32) && bestT_idx.alloc(npt) && bestT_dist.alloc(npt) && bestQ_idx.alloc(nk) && bestQ_dist.alloc(nk);
-    }
-    if (ok) {
-      ingest_ptr.adopt(blobG.h, blobG.d, B);
-      ingest_off.adopt(blobG.h + (size_t)B * 8, blobG.d + (size_t)B * 8, B);
-    }
-    if (ok) {  // the tracker-phase tables, carved out of one pinned + one device blob
-      const size_t nB = (size_t)B, npt = (size_t)B * max_pts, nnew = (size_t)B * e0.tc.num_features_max;
-      struct Sec { size_t bytes, off; };
-      Sec sec[14] = {{npt * 2 * 4, 0}, {nB * 8, 0}, {nB * 8, 0}, {nB * 8, 0}, {nB * 4, 0}, {nB * 8, 0}, {nB * 4, 0}, {nB * 4, 0}, {nB * 4, 0},  // pts0 off_cur off_prev fast_off npts frame_ptr ring_img pyr_img tkind
-                     {npt * 2 * 4, 0},                                                                                                   // pts1
-                     {npt, 0}, {nB * 4, 0}, {nB * 4, 0}, {nnew * 4, 0}};                                                                 // tstat tneed tnnew tnewkp
-      size_t off = 0;
-      for (Sec& q : sec) { q.off = off; off += (q.bytes + 15) & ~(size_t)15; }
-      ok = tt.alloc_fetchable((off + 15) & ~(size_t)15);
-      if (ok) {
-        auto H = [&](int i) { return (void*)(tt.h + sec[i].off); };
-        auto D = [&](int i) { return (void*)(tt.d + sec[i].off); };
-        pts0.adopt(H(0), D(0), npt * 2); off_cur.adopt(H(1), D(1), nB); off_prev.adopt(H(2), D(2), nB); fast_off.adopt(H(3), D(3), nB);
-        npts.adopt(H(4), D(4), nB); frame_ptr.adopt(H(5), D(5), nB); ring_img.adopt(H(6), D(6), nB); pyr_img.adopt(H(7), D(7), nB);
-        tkind.adopt(H(8), D(8), nB); pts1.adopt(H(9), D(9), npt * 2); tstat.adopt(H(10), D(10), npt); tneed.adopt(H(11), D(11), nB);
-        tnnew.adopt(H(12), D(12), nB); tnewkp.adopt(H(13), D(13), nnew);
-        tt_up_bytes = sec[10].off;  // inputs + pts1
-        tt_down_off = sec[9].off;   // pts1 + outputs
-        tt_down_bytes = off - sec[9].off;
-      }
-    }
+    // the tracker-phase tables: [inputs | pts1 (in/out) | outputs]; the upload covers inputs + pts1, the read-back pts1 + outputs
+    ok = ok && carve(tt, [&](BlobLayout& t) {
+           t.put(pts0, npt * 2); t.put(off_cur, nB); t.put(off_prev, nB); t.put(fast_off, nB); t.put(npts, nB); t.put(frame_ptr, nB);
+           t.put(ring_img, nB); t.put(pyr_img, nB); t.put(tkind, nB);
+           tt_down_off = t.put(pts1, npt * 2);
+           tt_up_bytes = t.put(tstat, npt);
+           t.put(tneed, nB); t.put(tnnew, nB); t.put(tnewkp, nB * e0.tc.num_features_max);
+           tt_down_bytes = t.off - tt_down_off;
+         });
     if (!ok) return fail(XIVO_ERR_CUDA, "device allocation for the image tracker failed");
     {  // TMA passes where the geometry allows (XIVO_PYRDOWN_TMA=0 / XIVO_FAST_TMA=0 keep the thread-staged kernels: parity tests compare the two)
       const char* tv = getenv("XIVO_PYRDOWN_TMA");
       const char* gv = getenv("XIVO_PYRDOWN_GENERIC");
       const char* fv = getenv("XIVO_FAST_TMA");
       if (cn == 1 && (cols & 15) == 0 && (pd.total & 15) == 0 && (pd.off[0] & 15) == 0 && !(fv && fv[0] == '0'))
-        tma_fast = make_fast_tensor_map(&tm_fast, dPyr + pd.off[0], rows, cols, pd.total, (unsigned long long)B * 2) == 0;
+        tma_fast = make_fast_tensor_map(&tm_fast, dPyr.p + pd.off[0], rows, cols, pd.total, (unsigned long long)B * 2) == 0;
       if (cn == 1 && (cols & 15) == 0 && (pd.total & 15) == 0 && pd.n_levels > 1 && !(tv && tv[0] == '0') && !(gv && gv[0] == '1')) {
-        if (make_pyr_tensor_map(&tm_ring, dRing, rows, cols, ib, (unsigned long long)B * ring_n) == 0) {
+        if (make_pyr_tensor_map(&tm_ring, dRing.p, rows, cols, ib, (unsigned long long)B * ring_n) == 0) {
           tma_pyr = true;
           for (int l = 1; l + 1 < pd.n_levels; ++l)
             tm_lvl_ok[l] = (pd.cols[l] & 15) == 0 && (pd.off[l] & 15) == 0 &&
-                           make_pyr_tensor_map(&tm_lvl[l], dPyr + pd.off[l], pd.rows[l], pd.cols[l], pd.total, (unsigned long long)B * 2) == 0;
+                           make_pyr_tensor_map(&tm_lvl[l], dPyr.p + pd.off[l], pd.rows[l], pd.cols[l], pd.total, (unsigned long long)B * 2) == 0;
         }
       }
     }
     ring_next.assign(B, 0);
-    ring_ev.resize(ring_n);
-    for (auto& e : ring_ev) cudaEventCreateWithFlags(&e, cudaEventDisableTiming);
+    ring_ev = std::vector<Event>(ring_n);
     prev_slot.assign(B, 0);
     for (auto& e : est) e->tracker_set_geometry(rows, cols, !dev_decide);
     img_ready = true;
@@ -914,7 +888,7 @@ class Batch {
       const int cur = 1 - prev_slot[b];
       off_cur.h[b] = ((size_t)b * 2 + cur) * pd.total;
       off_prev.h[b] = ((size_t)b * 2 + prev_slot[b]) * pd.total;
-      frame_ptr.h[b] = dRing + ((size_t)b * ring_n + slots[i]) * ib;  // consumed by the first pyrDown pass
+      frame_ptr.h[b] = dRing.p + ((size_t)b * ring_n + slots[i]) * ib;  // consumed by the first pyrDown pass
       if (tma_pyr) { ring_img.h[b] = b * ring_n + slots[i]; pyr_img.h[b] = b * 2 + cur; }
     }
     return 0;
@@ -924,12 +898,12 @@ class Batch {
     if (tma_pyr) {
       std::optional<ProfScope> ps;
       if (all_levels) ps.emplace("pyrdown", st1);
-      if (int rc = launch_pyrdown_tma(st1, tm_ring, ring_img.d, dPyr, 0, off_cur.d, pd, 0, 1, B)) return rc;
+      if (int rc = launch_pyrdown_tma(st1, tm_ring, ring_img.d, dPyr.p, 0, off_cur.d, pd, 0, 1, B)) return rc;
       for (int l = 1; all_levels && l + 1 < pd.n_levels; ++l) {
-        if (tm_lvl_ok[l]) { if (int rc = launch_pyrdown_tma(st1, tm_lvl[l], pyr_img.d, dPyr, 0, off_cur.d, pd, l, 0, B)) return rc; }
-        else if (int rc = launch_pyrdown_level(st1, dPyr, 0, off_cur.d, pd, B, nullptr, l)) return rc;
+        if (tm_lvl_ok[l]) { if (int rc = launch_pyrdown_tma(st1, tm_lvl[l], pyr_img.d, dPyr.p, 0, off_cur.d, pd, l, 0, B)) return rc; }
+        else if (int rc = launch_pyrdown_level(st1, dPyr.p, 0, off_cur.d, pd, B, nullptr, l)) return rc;
       }
-    } else if (int rc = all_levels ? launch_build_pyramid(st1, dPyr, 0, off_cur.d, pd, B, frame_ptr.d) : launch_pyrdown_level(st1, dPyr, 0, off_cur.d, pd, B, frame_ptr.d, 0))
+    } else if (int rc = all_levels ? launch_build_pyramid(st1, dPyr.p, 0, off_cur.d, pd, B, frame_ptr.d) : launch_pyrdown_level(st1, dPyr.p, 0, off_cur.d, pd, B, frame_ptr.d, 0))
       return rc;
     g_launches += all_levels ? std::max(1, pd.n_levels - 1) : 1;
     return 0;
@@ -938,7 +912,7 @@ class Batch {
   int detect_and_fetch(const std::vector<int>& seqs, const unsigned long long* sel) {
     cudaStream_t st = st1;
     const TrackerCfg& tc = est[0]->tc;
-    if (int rc = launch_fast_detect(st, dPyr, 0, sel, rows, cols, cn, tc.fast_threshold, tc.fast_nonmax, kp.d, max_kp, kpcount.d, B, nullptr,
+    if (int rc = launch_fast_detect(st, dPyr.p, 0, sel, rows, cols, cn, tc.fast_threshold, tc.fast_nonmax, kp.d, max_kp, kpcount.d, B, nullptr,
                                     tma_fast ? &tm_fast : nullptr, pd.total))
       return rc;
     g_launches += 1;
@@ -954,7 +928,7 @@ class Batch {
   // LK of the staged points (pts0 -> pts1) from the previous to the current pyramid of every sequence with npts > 0
   int track_lk(const std::vector<int>& lk_list) {
     const TrackerCfg& tc = est[0]->tc;
-    if (int rc = launch_lk_track(st1, dPyr, dPyr, 0, off_prev.d, off_cur.d, pd, pts0.d, pts1.d, lkst.d, lkerr.d, npts.d, max_pts, B, tc.win_size, tc.max_iter,
+    if (int rc = launch_lk_track(st1, dPyr.p, dPyr.p, 0, off_prev.d, off_cur.d, pd, pts0.d, pts1.d, lkst.d, lkerr.d, npts.d, max_pts, B, tc.win_size, tc.max_iter,
                                  tc.eps, 1, 1e-4))
       return rc;
     g_launches += 1;
@@ -991,7 +965,7 @@ class Batch {
       }
     }
     XB_CUDA(nkps.up(st)); XB_CUDA(nq.up(st));
-    if (int rc = launch_brief(st, dPyr, 0, sel_off_dev, rows, cols, cn, kpxy.d, nkps.d, max_kp, descK.d, validK.d, B)) return rc;
+    if (int rc = launch_brief(st, dPyr.p, 0, sel_off_dev, rows, cols, cn, kpxy.d, nkps.d, max_kp, descK.d, validK.d, B)) return rc;
     g_launches += 1;
     if (any_q) {
       if (int rc = launch_hamming_nearest(st, qdesc.d, nq.d, max_pts, descK.d, nkps.d, max_kp, bestT_idx.d, bestT_dist.d, B)) return rc;
@@ -1034,7 +1008,7 @@ class Batch {
     }
     std::unique_ptr<HostScope> hx_fs(new HostScope("x_i_trk_fast_select"));
     // FAST on the current level-0 image of every tracked sequence (fast_off); the kernel skips those whose need is 0
-    if (int rc = launch_fast_detect(st, dPyr, 0, fast_off.d, rows, cols, cn, tc.fast_threshold, tc.fast_nonmax, kp.d, max_kp, kpcount.d, B, tneed.d,
+    if (int rc = launch_fast_detect(st, dPyr.p, 0, fast_off.d, rows, cols, cn, tc.fast_threshold, tc.fast_nonmax, kp.d, max_kp, kpcount.d, B, tneed.d,
                                     tma_fast ? &tm_fast : nullptr, pd.total, true))
       return rc;
     if (int rc = launch_track_select(st, dc, tkind.d, npts.d, pts1.d, tstat.d, tneed.d, kp.d, kpcount.d, tnewkp.d, tnnew.d, B)) return rc;
@@ -1112,7 +1086,7 @@ class Batch {
       if (int rc = track_lk(lk_list)) return rc;
       XB_CUDA(pts1.down(st)); XB_CUDA(lkst.down(st));
       if (desc_on) {  // descriptors at the tracked positions (tracker.cpp:530-545), same stream, same wait
-        if (int rc = launch_brief(st, dPyr, 0, off_cur.d, rows, cols, cn, pts1.d, npts.d, max_pts, descT.d, validT.d, B)) return rc;
+        if (int rc = launch_brief(st, dPyr.p, 0, off_cur.d, rows, cols, cn, pts1.d, npts.d, max_pts, descT.d, validT.d, B)) return rc;
         g_launches += 1;
         XB_CUDA(descT.down(st)); XB_CUDA(validT.down(st));
       }
@@ -1193,9 +1167,9 @@ class Batch {
     std::vector<int> act;
     for (int b : full)
       if (est[b]->ransac.active) act.push_back(b);
-    if (!dP0) XB_CUDA(cudaMalloc(reinterpret_cast<void**>(&dP0), sizeof(double) * B * N * N));
+    if (!dP0.p && !dP0.alloc((size_t)B * N * N)) return fail(XIVO_ERR_CUDA, "1-point RANSAC: covariance backup allocation failed");
     for (int b : act)  // BackupState
-      XB_CUDA(cudaMemcpyAsync(dP0 + (size_t)b * N * N, dP + (size_t)b * N * N, sizeof(double) * N * N, cudaMemcpyDeviceToDevice, st));
+      XB_CUDA(cudaMemcpyAsync(dP0.p + (size_t)b * N * N, dP.p + (size_t)b * N * N, sizeof(double) * N * N, cudaMemcpyDeviceToDevice, st));
     // ---- phase 1: the low-innovation update
     for (int b = 0; b < B; ++b) { nsel.h[b] = 0; nopsU.h[b] = 0; firstU.h[b] = 0; }
     int nops_total = 0;
@@ -1214,8 +1188,8 @@ class Batch {
       nsel.h[b] = k;
     }
     XB_CUDA(up_blob(blobU, blobU_fixed + (size_t)nops_total * sizeof(EditOp), st));
-    if (int rc = launch_ekf_update(st, lay, dJac, sel.d, nsel.d, R.d, dP, dErr, dHP, dKt, nullptr, B, 0, opsU.d, firstU.d, nopsU.d, nullptr, 1)) return rc;
-    if (int rc = launch_pack_state(st, N, dP, dErr, pack.d, B)) return rc;
+    if (int rc = launch_ekf_update(st, lay, dJac.p, sel.d, nsel.d, R.d, dP.p, dErr.p, dHP.p, dKt.p, nullptr, B, 0, opsU.d, firstU.d, nopsU.d, nullptr, 1)) return rc;
+    if (int rc = launch_pack_state(st, N, dP.p, dErr.p, pack.d, B)) return rc;
     g_launches += 3;
     XB_CUDA(pack.down(st));
     if (int rc = wait(st)) return rc;
@@ -1234,13 +1208,13 @@ class Batch {
     for (int b : act) nfeat.h[b] = nfeat_saved[b];
     XB_CUDA(up_blob(blobS, blobS_fixed, st));
     XB_CUDA(up_blob(blobJ, blobJ_fixed, st));
-    if (int rc = launch_jacobian_gate(st, lay, cam.d, X.d, groups.d, fx.d, fxp.d, fref.d, fsind.d, nfeat.d, dP, R.d, dJac, nullptr, mh.d, B, opsJ.d, firstJ.d, nopsJ.d,
+    if (int rc = launch_jacobian_gate(st, lay, cam.d, X.d, groups.d, fx.d, fxp.d, fref.d, fsind.d, nfeat.d, dP.p, R.d, dJac.p, nullptr, mh.d, B, opsJ.d, firstJ.d, nopsJ.d,
                                       nullptr))
       return rc;
     g_launches += 1;
     XB_CUDA(mh.down(st, (size_t)B * lay.F));
     for (int b : act)  // RestoreState (stream order: after the kernel above)
-      XB_CUDA(cudaMemcpyAsync(dP + (size_t)b * N * N, dP0 + (size_t)b * N * N, sizeof(double) * N * N, cudaMemcpyDeviceToDevice, st));
+      XB_CUDA(cudaMemcpyAsync(dP.p + (size_t)b * N * N, dP0.p + (size_t)b * N * N, sizeof(double) * N * N, cudaMemcpyDeviceToDevice, st));
     if (int rc = wait(st)) return rc;
     for (int b : act) est[b]->ransac_finish(mh.h + (size_t)b * lay.F, table_order[b]);
     if (int rc = first_error(full)) return rc;
@@ -1259,7 +1233,7 @@ class Batch {
     }
     XB_CUDA(up_blob(blobS, blobS_fixed, st));
     XB_CUDA(up_blob(blobJ, blobJ_fixed, st));  // (nfeat still selects the active sequences only)
-    if (int rc = launch_jacobian_gate(st, lay, cam.d, X.d, groups.d, fx.d, fxp.d, fref.d, fsind.d, nfeat.d, dP, R.d, dJac, nullptr, mh.d, B, opsJ.d, firstJ.d, nopsJ.d,
+    if (int rc = launch_jacobian_gate(st, lay, cam.d, X.d, groups.d, fx.d, fxp.d, fref.d, fsind.d, nfeat.d, dP.p, R.d, dJac.p, nullptr, mh.d, B, opsJ.d, firstJ.d, nopsJ.d,
                                       nullptr))
       return rc;
     g_launches += 1;
@@ -1401,7 +1375,7 @@ class Batch {
     std::unique_ptr<HostScope> hs_issue(new HostScope("issue_jacobian"));
     // one copy: [nfeat | nops | first | fref | fsind | fxp | fx | groups | packed edit list]; the kernel applies the edits, then the features
     XB_CUDA(up_blob(blobJ, blobJ_fixed + (size_t)nops_total * sizeof(EditOp), st));
-    if (int rc = launch_jacobian_gate(st, lay, cam.d, X.d, groups.d, fx.d, fxp.d, fref.d, fsind.d, nfeat.d, dP, R.d, dJac, nullptr, mh.d, B, opsJ.d,
+    if (int rc = launch_jacobian_gate(st, lay, cam.d, X.d, groups.d, fx.d, fxp.d, fref.d, fsind.d, nfeat.d, dP.p, R.d, dJac.p, nullptr, mh.d, B, opsJ.d,
                                       firstJ.d, nopsJ.d, use_1pt ? mh.d + (size_t)B * lay.F : nullptr))
       return rc;
     g_launches += 1;
@@ -1450,8 +1424,8 @@ class Batch {
     }
     hs_issue.reset(new HostScope("issue_update"));
     XB_CUDA(up_blob(blobU, blobU_fixed + (size_t)nops_total * sizeof(EditOp), st));  // [nsel | nops | first | sel | packed post-gate edit list]
-    if (int rc = launch_ekf_update(st, lay, dJac, sel.d, nsel.d, R.d, dP, dErr, dHP, dKt, nullptr, B, cov_tc, opsU.d, firstU.d, nopsU.d, dKt32 ? &tcops : nullptr)) return rc;
-    if (int rc = launch_pack_state(st, N, dP, dErr, pack.d, B)) return rc;
+    if (int rc = launch_ekf_update(st, lay, dJac.p, sel.d, nsel.d, R.d, dP.p, dErr.p, dHP.p, dKt.p, nullptr, B, cov_tc, opsU.d, firstU.d, nopsU.d, dKt32.p ? &tcops : nullptr)) return rc;
+    if (int rc = launch_pack_state(st, N, dP.p, dErr.p, pack.d, B)) return rc;
     g_launches += 3;
     for (int b : full) {
       const double M = 2.0 * nsel.h[b], Nn = N;
@@ -1778,14 +1752,14 @@ int xivo_get_P(xivo_batch* b, int seq, double* out) {
   BATCH_BEGIN; SEQ_CHECK;
   XB_REQUIRE(out, "get_P: null output");
   if (int rc = B_.flush({seq})) return rc;
-  XB_CUDA(cudaMemcpy(out, B_.dP + (size_t)seq * B_.N * B_.N, sizeof(double) * B_.N * B_.N, cudaMemcpyDeviceToHost));
+  XB_CUDA(cudaMemcpy(out, B_.dP.p + (size_t)seq * B_.N * B_.N, sizeof(double) * B_.N * B_.N, cudaMemcpyDeviceToHost));
   return 0;
 }
 int xivo_get_Pstate(xivo_batch* b, int seq, double* out81) {
   BATCH_BEGIN; SEQ_CHECK;
   if (int rc = B_.flush({seq})) return rc;
   for (int i = 0; i < 9; ++i)
-    XB_CUDA(cudaMemcpy(out81 + 9 * i, B_.dP + (size_t)seq * B_.N * B_.N + (size_t)i * B_.N, sizeof(double) * 9, cudaMemcpyDeviceToHost));
+    XB_CUDA(cudaMemcpy(out81 + 9 * i, B_.dP.p + (size_t)seq * B_.N * B_.N + (size_t)i * B_.N, sizeof(double) * 9, cudaMemcpyDeviceToHost));
   return 0;
 }
 int xivo_get_counters(xivo_batch* b, int seq, int* out) {
@@ -1878,7 +1852,7 @@ int xivo_get_instate_groups(xivo_batch* b, int seq, int* ids, int* sinds, double
 static int fetch_P(Batch& B_, int seq, std::vector<double>* P) {
   P->resize((size_t)B_.N * B_.N);
   if (int rc = B_.flush({seq})) return rc;
-  XB_CUDA(cudaMemcpy(P->data(), B_.dP + (size_t)seq * B_.N * B_.N, sizeof(double) * B_.N * B_.N, cudaMemcpyDeviceToHost));
+  XB_CUDA(cudaMemcpy(P->data(), B_.dP.p + (size_t)seq * B_.N * B_.N, sizeof(double) * B_.N * B_.N, cudaMemcpyDeviceToHost));
   return 0;
 }
 int xivo_get_instate_feature_table(xivo_batch* b, int seq, int n_output, int* ids, int* sinds, int* ref_group_ids, double* Xs3, double* Xc3,
