@@ -5,18 +5,162 @@
 // (file name ending in .png) go through Estimator::VisualMeas(ts, path), decoded on the device like cv::imread(path).
 // `--list` stops after loading and prints the merged message list (used by the CPU test of the loader); for a PNG frame it prints
 // the file's geometry (xivo_png_info) and size in bytes instead of the pixel checksum.
+//   vio --batch <estimator_cfg.json> <list.txt> [max_groups max_features]
+// runs every sequence of list.txt in one xivo::Batch handle.  Each line of the list is `image_dir imu_dir out_state [cfg.json]` (empty
+// lines and lines starting with '#' are skipped); a line's own config, which must agree with the handle's on the batch-wide settings,
+// is applied with ResetSequence before the first message.  Round r gives every sequence its r-th piece (xivo::FeedPieces: its IMU
+// messages up to and including its next frame), PNM frames through Batch::Feed and PNG frames through Batch::FeedPng, and after each
+// round the trajectory line of every sequence that received a frame is written to its out_state: the lines a solo run writes at
+// that sequence's frame messages.  `--batch --plan <list.txt>` stops after loading and prints one line per piece:
+// `round sequence n_imu frame_ts` (`-` for a piece without a frame).
 // Build: g++ -std=c++17 -O2 -I include examples/vio.cpp -o vio -L xivo_b200 -lxivo_b200 -Wl,-rpath,$PWD/xivo_b200
 #include <cstdio>
 #include <cstring>
 #include <fstream>
 #include <iostream>
+#include <iterator>
+#include <memory>
+#include <sstream>
+#include <string>
+#include <vector>
 
 #include "xivo_b200.hpp"
 #include "xivo_b200_io.hpp"
 
 static bool is_png(const std::string& p) { return p.size() >= 4 && p.compare(p.size() - 4, 4, ".png") == 0; }
 
+static std::string read_text(const std::string& path) {
+  std::ifstream f(path);
+  if (!f) throw std::runtime_error("cannot open " + path);
+  return std::string((std::istreambuf_iterator<char>(f)), std::istreambuf_iterator<char>());
+}
+
+struct SeqLine {
+  std::string image_dir, imu_dir, out_state, cfg;
+};
+
+static std::vector<SeqLine> read_list(const std::string& path) {
+  std::ifstream f(path);
+  if (!f) throw std::runtime_error("cannot open " + path);
+  std::vector<SeqLine> out;
+  std::string line;
+  while (std::getline(f, line)) {
+    std::istringstream ss(line);
+    SeqLine l;
+    if (!(ss >> l.image_dir) || l.image_dir[0] == '#') continue;
+    if (!(ss >> l.imu_dir >> l.out_state)) throw std::runtime_error(path + ": a line needs image_dir imu_dir out_state [cfg.json]: " + line);
+    ss >> l.cfg;
+    out.push_back(l);
+  }
+  if (out.empty()) throw std::runtime_error(path + " lists no sequence");
+  return out;
+}
+
+static int run_batch(int argc, char** argv) {
+  const bool plan = argc >= 4 && !std::strcmp(argv[2], "--plan");
+  if (argc < 4) {
+    std::fprintf(stderr, "usage: %s --batch <estimator_cfg.json> <list.txt> [max_groups max_features] | --batch --plan <list.txt>\n", argv[0]);
+    return 1;
+  }
+  const std::vector<SeqLine> list = read_list(argv[3]);
+  const int B = (int)list.size();
+  std::vector<std::unique_ptr<xivo::DataLoader>> loaders;
+  std::vector<std::vector<std::pair<int, int>>> pieces;
+  size_t rounds = 0;
+  for (const auto& l : list) {
+    loaders.emplace_back(new xivo::DataLoader(l.image_dir, l.imu_dir));
+    pieces.push_back(xivo::FeedPieces(*loaders.back()));
+    rounds = std::max(rounds, pieces.back().size());
+  }
+  auto frame_of = [&](int s, size_t r) -> const xivo::msg::Image* {  // the frame ending sequence s's piece r, or null
+    if (r >= pieces[s].size()) return nullptr;
+    return dynamic_cast<const xivo::msg::Image*>(loaders[s]->Get(pieces[s][r].second - 1));
+  };
+  if (plan) {
+    for (size_t r = 0; r < rounds; ++r)
+      for (int s = 0; s < B; ++s) {
+        if (r >= pieces[s].size()) continue;
+        const auto* im = frame_of(s, r);
+        const int n_imu = pieces[s][r].second - pieces[s][r].first - (im ? 1 : 0);
+        if (im) std::printf("%zu %d %d %lld\n", r, s, n_imu, (long long)im->ts_ns);
+        else std::printf("%zu %d %d -\n", r, s, n_imu);
+      }
+    return 0;
+  }
+  const int G = argc > 5 ? std::atoi(argv[4]) : 15, F = argc > 5 ? std::atoi(argv[5]) : 30;
+  xivo::Batch batch(read_text(argv[2]), B, G, F);
+  std::vector<std::ofstream> out(B);
+  for (int s = 0; s < B; ++s) {
+    if (!list[s].cfg.empty()) {
+      try {
+        batch.ResetSequence(s, read_text(list[s].cfg));
+      } catch (const xivo::Error& e) {
+        throw xivo::Error(e.code, list[s].cfg + ": " + e.what());
+      }
+    }
+    out[s].open(list[s].out_state);
+    if (!out[s]) throw std::runtime_error("cannot write " + list[s].out_state);
+  }
+  for (size_t r = 0; r < rounds; ++r) {
+    std::vector<xivo::Batch::Input> pnm(B), png(B);
+    std::vector<xivo::PnmImage> pixels(B);
+    bool any_pnm = false, any_png = false;
+    for (int s = 0; s < B; ++s) {
+      if (r >= pieces[s].size()) continue;
+      xivo::Batch::Input& in = pnm[s];  // the IMU samples go with the first call of the round
+      for (int i = pieces[s][r].first; i < pieces[s][r].second; ++i)
+        if (auto* mu = dynamic_cast<const xivo::msg::IMU*>(loaders[s]->Get(i))) {
+          in.imu_ts.push_back((uint64_t)mu->ts_ns);
+          in.gyro.push_back({mu->gyro_[0], mu->gyro_[1], mu->gyro_[2]});
+          in.accel.push_back({mu->accel_[0], mu->accel_[1], mu->accel_[2]});
+        }
+      const auto* im = frame_of(s, r);
+      if (!im) continue;
+      if (is_png(im->image_path_)) {
+        png[s].has_frame = any_png = true;
+        png[s].frame_ts = (uint64_t)im->ts_ns;
+        png[s].png = xivo::ReadFileBytes(im->image_path_);
+      } else {
+        pixels[s] = xivo::ReadPnm(im->image_path_);
+        in.has_frame = any_pnm = true;
+        in.frame_ts = (uint64_t)im->ts_ns;
+        in.image = xivo::ImageView{pixels[s].data.data(), pixels[s].rows, pixels[s].cols, pixels[s].channels};
+      }
+    }
+    if (any_pnm || !any_png) batch.Feed(pnm);
+    if (any_png) {
+      if (!any_pnm)  // the round's only call carries the IMU samples
+        for (int s = 0; s < B; ++s) {
+          png[s].imu_ts.swap(pnm[s].imu_ts);
+          png[s].gyro.swap(pnm[s].gyro);
+          png[s].accel.swap(pnm[s].accel);
+        }
+      batch.FeedPng(png);
+    }
+    for (int s = 0; s < B; ++s)
+      if (frame_of(s, r)) {
+        const auto g = batch.gsb(s);
+        out[s] << xivo::TrajectoryLine(batch.ts(s).count(), g.data()) << "\n";
+      }
+  }
+  for (int s = 0; s < B; ++s)
+    std::printf("sequence %d: %d messages, %d in-state features, %d groups\n", s, loaders[s]->size(), batch.num_instate_features(s),
+                batch.num_instate_groups(s));
+  return 0;
+}
+
 int main(int argc, char** argv) {
+  if (argc >= 2 && !std::strcmp(argv[1], "--batch")) {
+    try {
+      return run_batch(argc, argv);
+    } catch (const xivo::Error& e) {
+      std::fprintf(stderr, "xivo::Error %d: %s\n", e.code, e.what());
+      return e.code == XIVO_ERR_CUDA ? 42 : 3;
+    } catch (const std::exception& e) {
+      std::fprintf(stderr, "%s\n", e.what());
+      return 2;
+    }
+  }
   if (argc >= 4 && !std::strcmp(argv[1], "--list")) {
     try {
       xivo::DataLoader loader(argv[2], argv[3]);

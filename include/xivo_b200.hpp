@@ -313,6 +313,106 @@ class Estimator {
   bool tracker_only_ = false;
 };
 
+// One handle of n independent sequences, each fed its own messages per call (xivo_batch_feed / xivo_batch_feed_png): recorded
+// sequences with different start times, lengths, IMU rates and dropped frames run side by side, every one of them bit-identical to an
+// Estimator fed the same messages one at a time.  Getters take the sequence index.
+class Batch {
+ public:
+  // What one sequence receives in one Feed / FeedPng call: its IMU samples in order, then at most one frame.
+  struct Input {
+    std::vector<uint64_t> imu_ts;
+    std::vector<Vec3> gyro, accel;
+    bool has_frame = false;
+    uint64_t frame_ts = 0;
+    ImageView image{nullptr, 0, 0, 0};  // Feed
+    std::vector<uint8_t> png;            // FeedPng: the PNG file's bytes
+  };
+
+  Batch(const std::string& cfg_json, int n_seq, int max_groups, int max_features, bool tracker_only = false, int device = 0) {
+    if (int rc = xivo_ctx_create(device, &ctx_)) throw Error(rc, xivo_last_error());
+    if (int rc = xivo_batch_create(ctx_, cfg_json.c_str(), n_seq, max_groups, max_features, tracker_only ? 1 : 0, &b_)) {
+      const std::string msg = xivo_last_error();
+      xivo_ctx_destroy(ctx_);
+      throw Error(rc, msg);
+    }
+    n_ = n_seq;
+  }
+  ~Batch() {
+    if (b_) xivo_batch_destroy(b_);
+    if (ctx_) xivo_ctx_destroy(ctx_);
+  }
+  Batch(const Batch&) = delete;
+  Batch& operator=(const Batch&) = delete;
+  int size() const { return n_; }
+
+  // in[s] for every sequence s; the frames are image views of one geometry
+  void Feed(const std::vector<Input>& in, bool tracker_only = false) {
+    Flat f = flatten(in);
+    std::vector<const uint8_t*> imgs(n_, nullptr);
+    int rows = 0, cols = 0, ch = 0;
+    for (int s = 0; s < n_; ++s)
+      if (in[s].has_frame) {
+        imgs[s] = in[s].image.data;
+        rows = in[s].image.rows; cols = in[s].image.cols; ch = in[s].image.channels;
+      }
+    check(xivo_batch_feed(b_, f.n_imu.data(), f.ts.data(), f.gyro.data(), f.accel.data(), f.frame_ts.data(), imgs.data(), rows, cols, ch, 0,
+                          tracker_only ? 1 : 0));
+  }
+  // the same with PNG frames (Input::png), decoded on the device like cv::imread (channels = 3: BGR)
+  void FeedPng(const std::vector<Input>& in, int channels = 3, bool tracker_only = false) {
+    Flat f = flatten(in);
+    std::vector<const uint8_t*> png(n_, nullptr);
+    std::vector<size_t> bytes(n_, 0);
+    for (int s = 0; s < n_; ++s)
+      if (in[s].has_frame) { png[s] = in[s].png.data(); bytes[s] = in[s].png.size(); }
+    check(xivo_batch_feed_png(b_, f.n_imu.data(), f.ts.data(), f.gyro.data(), f.accel.data(), f.frame_ts.data(), png.data(), bytes.data(), channels,
+                              tracker_only ? 1 : 0));
+  }
+  // sequence `seq` starts over, with the handle's config (cfg_json empty) or a compatible one of its own (xivo_batch_reset_sequence)
+  void ResetSequence(int seq, const std::string& cfg_json = std::string()) {
+    check(xivo_batch_reset_sequence(b_, seq, cfg_json.empty() ? nullptr : cfg_json.c_str()));
+  }
+
+  Mat34 gsb(int seq) const { Mat34 g; check(xivo_get_gsb(b_, seq, g.data())); return g; }
+  timestamp_t ts(int seq) const { uint64_t t = 0; check(xivo_get_time_ns(b_, seq, &t)); return timestamp_t((int64_t)t); }
+  int num_instate_features(int seq) const { return counters(seq)[0]; }
+  int num_instate_groups(int seq) const { return counters(seq)[1]; }
+  xivo_batch* handle() { return b_; }
+
+ private:
+  struct Flat { std::vector<int> n_imu; std::vector<uint64_t> ts, frame_ts; std::vector<double> gyro, accel; };
+  Flat flatten(const std::vector<Input>& in) const {
+    if ((int)in.size() != n_) throw Error(XIVO_ERR_ARG, "Batch: expected one Input per sequence");
+    Flat f;
+    f.n_imu.resize(n_);
+    f.frame_ts.assign(n_, 0);
+    for (int s = 0; s < n_; ++s) {
+      const Input& x = in[s];
+      if (x.gyro.size() != x.imu_ts.size() || x.accel.size() != x.imu_ts.size())
+        throw Error(XIVO_ERR_ARG, "Batch: sequence " + std::to_string(s) + ": IMU stamps, gyro and accel differ in length");
+      f.n_imu[s] = (int)x.imu_ts.size();
+      f.ts.insert(f.ts.end(), x.imu_ts.begin(), x.imu_ts.end());
+      for (size_t k = 0; k < x.imu_ts.size(); ++k) {
+        f.gyro.insert(f.gyro.end(), x.gyro[k].begin(), x.gyro[k].end());
+        f.accel.insert(f.accel.end(), x.accel[k].begin(), x.accel[k].end());
+      }
+      if (x.has_frame) f.frame_ts[s] = x.frame_ts;
+    }
+    return f;
+  }
+  void check(int rc) const {
+    if (rc) throw Error(rc, xivo_last_error());
+  }
+  std::array<int, XIVO_NUM_COUNTERS> counters(int seq) const {
+    std::array<int, XIVO_NUM_COUNTERS> c;
+    check(xivo_get_counters(b_, seq, c.data()));
+    return c;
+  }
+  xivo_ctx* ctx_ = nullptr;
+  xivo_batch* b_ = nullptr;
+  int n_ = 0;
+};
+
 // Kernel-level Tracker facade: the OpenCV calls of Tracker::DetectLK / UpdateLK (src/tracker.cpp:224, :476-528) on
 // caller-owned images.  The stateful tracker (feature list, mask, redetection) lives inside xivo::Estimator, as it does
 // behind Estimator::VisualMeas in the reference.

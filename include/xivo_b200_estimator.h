@@ -71,6 +71,24 @@ int xivo_batch_visual_meas_device(xivo_batch* b, const uint64_t* ts_ns, const ui
 int xivo_batch_step(xivo_batch* b, int n_imu, const uint64_t* imu_ts, const double* gyro, const double* accel,
                     const uint64_t* frame_ts, const uint8_t* const* imgs, int rows, int cols, int channels, int on_device);
 
+/* Per-sequence input for one call, for sequences whose message patterns differ (start times, lengths, IMU samples per frame, dropped
+ * frames).  Sequence s receives n_imu[s] InertialMeas, in the order given, then at most one VisualMeas (or VisualMeasTrackerOnly).  Its IMU
+ * rows are at offset sum(n_imu[0..s-1]) of imu_ts / gyro (x 3) / accel (x 3).  imgs[s] == NULL (or imgs == NULL): no frame for s;
+ * frame_ts[s] is read only where there is a frame.  A sequence with n_imu[s] == 0 and no frame is not touched.
+ * After the call every sequence is bit-identical to sequence 0 of a one-sequence handle (same config, G, F, tracker_only) given the same
+ * messages one at a time; xivo_batch_step is the case where every sequence has the same n_imu and a frame.  Only the sequences with a
+ * frame take a ring slot, so one frame per sequence per call keeps the ring bound.  on_device != 0: imgs are device pointers.  Pending
+ * xivo_batch_prefetch_frames uploads are dropped, as for any call with other buffers.
+ * Refused with XIVO_ERR_ARG naming the sequence before any message is pushed (nothing changes): a negative n_imu, NULL IMU arrays while
+ * some n_imu[s] > 0, a frame geometry other than the handle's.  XIVO_ERR_STATE once an earlier call on the handle failed. */
+int xivo_batch_feed(xivo_batch* b, const int* n_imu, const uint64_t* imu_ts, const double* gyro, const double* accel,
+                    const uint64_t* frame_ts, const uint8_t* const* imgs, int rows, int cols, int channels, int on_device, int tracker_only);
+/* The same, with frames as PNG files (png[s] == NULL: no frame for s), decoded on the device as in xivo_batch_visual_meas_png; only the
+ * present frames are parsed, uploaded and decoded.  A refused or corrupt file of any sequence returns XIVO_ERR_ARG naming it before any
+ * message is pushed: no sequence changes and the handle stays usable. */
+int xivo_batch_feed_png(xivo_batch* b, const int* n_imu, const uint64_t* imu_ts, const double* gyro, const double* accel,
+                        const uint64_t* frame_ts, const uint8_t* const* png, const size_t* png_bytes, int channels, int tracker_only);
+
 /* Optional streaming hint: start the host->device copy of the NEXT frame of every sequence now, so that it
  * overlaps the step that is still being computed (the reference decouples acquisition from estimation the same
  * way, with its message queue: /root/reference/src/estimator_process.cpp).  Up to two prefetched frames may

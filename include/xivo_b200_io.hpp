@@ -15,6 +15,7 @@
 #include <sstream>
 #include <stdexcept>
 #include <string>
+#include <utility>
 #include <vector>
 
 namespace xivo {
@@ -91,6 +92,20 @@ class DataLoader {
     std::stable_sort(entries_.begin(), entries_.end(), [](const auto& a, const auto& b) { return a->ts_ns < b->ts_ns; });
   }
 };
+// The pieces of a loaded sequence for xivo::Batch::Feed, as [begin, end) message ranges: the IMU messages up to and including the next
+// image, and the IMU messages after the last image as a last piece.  Round r of a batch gives every sequence its r-th piece
+// (xivo_b200.dataio.feed_rounds is the same rule in Python).
+inline std::vector<std::pair<int, int>> FeedPieces(const DataLoader& loader) {
+  std::vector<std::pair<int, int>> out;
+  int begin = 0;
+  for (int i = 0; i < loader.size(); ++i)
+    if (dynamic_cast<const msg::Image*>(loader.Get(i))) {
+      out.emplace_back(begin, i + 1);
+      begin = i + 1;
+    }
+  if (begin < loader.size()) out.emplace_back(begin, loader.size());
+  return out;
+}
 using TUMVILoader = DataLoader;
 using EuRoCLoader = DataLoader;
 

@@ -399,11 +399,7 @@ class Batch {
   // sequences, their heaps and their frames in the ring are untouched.  Refused without any change when an earlier call failed, when
   // the config does not parse or when it differs from the handle in a batch-wide setting (batch_incompatibility).
   int reset_sequence(int seq, const Json* cfg) {
-    if (pfor_bad.load()) return fail(XIVO_ERR_STATE, "reset_sequence: an earlier call on this handle failed (" + pfor_msg + "); the handle cannot continue");
-    for (int b = 0; b < B; ++b)
-      if (est[b]->error)
-        return fail(XIVO_ERR_STATE, "reset_sequence: an earlier call on this handle failed (sequence " + std::to_string(b) + ": " + est[b]->error_msg +
-                                        "); the handle cannot continue");
+    if (int rc = refuse_if_failed("reset_sequence")) return rc;
     std::unique_ptr<Estimator> e;
     try {
       e.reset(new Estimator(cfg ? *cfg : cfg0, lay, est[0]->tracker_only));
@@ -424,10 +420,7 @@ class Batch {
     }
     est[seq] = std::move(e);  // the old estimator's heap, pending propagation records, edits and tracker state go with it
     table_order[seq].clear();
-    if (!pref.empty()) {  // pending prefetches are dropped as take_slots drops them: their slots are handed out again
-      for (int s = 0; s < B; ++s) ring_next[s] = pref.front().slot[s];
-      pref.clear();
-    }
+    drop_prefetches();
     set_filter_tables(seq);
     // Device side on st2, in stream order behind the work already queued for the old sequence (an imu_cov_propagate of a frame the heap
     // has released reads icst and P), ahead of everything the new one enqueues.
@@ -450,6 +443,20 @@ class Batch {
   int fail(int code, const std::string& m) {
     set_error("%s", m.c_str());
     return code;
+  }
+  // XIVO_ERR_STATE once an earlier call on the handle failed: such a call stops mid-frame for every sequence
+  int refuse_if_failed(const char* what) {
+    if (pfor_bad.load()) return fail(XIVO_ERR_STATE, std::string(what) + ": an earlier call on this handle failed (" + pfor_msg + "); the handle cannot continue");
+    for (int b = 0; b < B; ++b)
+      if (est[b]->error)
+        return fail(XIVO_ERR_STATE, std::string(what) + ": an earlier call on this handle failed (sequence " + std::to_string(b) + ": " + est[b]->error_msg +
+                                        "); the handle cannot continue");
+    return 0;
+  }
+  std::vector<int> every_sequence() const {
+    std::vector<int> all(B);
+    for (int s = 0; s < B; ++s) all[s] = s;
+    return all;
   }
 
   // ---- staging helpers -------------------------------------------------------------------
@@ -615,16 +622,23 @@ class Batch {
     }
     return static_cast<const uint8_t*>(at.devicePointer);
   }
-  // Ring slots of the frame about to be ingested.  If the oldest pending xivo_batch_prefetch_frames call brought exactly these host buffers,
-  // their upload is already enqueued (*uploaded = true) and its slots are taken over; otherwise every pending prefetch is abandoned and its
-  // slots are handed out again (st_copy is in order: the new upload lands after the abandoned ones).
-  void fresh_slots(std::vector<int>& slot_of) {
-    for (int s = 0; s < B; ++s) {
+  // The next ring slot of every sequence in `seqs` (slot_of is indexed by sequence; the others' entries are left alone).
+  void fresh_slots(const std::vector<int>& seqs, std::vector<int>& slot_of) {
+    for (int s : seqs) {
       const int slot = ring_next[s];
       ring_next[s] = (slot + 1) % ring_n;
       slot_of[s] = slot;
     }
   }
+  // pending prefetches are abandoned and their slots handed out again (st_copy is in order: a new upload lands after the abandoned ones)
+  void drop_prefetches() {
+    if (pref.empty()) return;
+    for (int s = 0; s < B; ++s) ring_next[s] = pref.front().slot[s];
+    pref.clear();
+  }
+  // Ring slots of the frame about to be ingested.  If the oldest pending xivo_batch_prefetch_frames call brought exactly these host buffers,
+  // their upload is already enqueued (*uploaded = true) and its slots are taken over; otherwise every pending prefetch is abandoned and its
+  // slots are handed out again (st_copy is in order: the new upload lands after the abandoned ones).
   void take_slots(const uint8_t* const* imgs, bool on_device, std::vector<int>& slot_of, bool* uploaded) {
     bool match = !pref.empty() && !on_device;
     if (match)
@@ -636,70 +650,76 @@ class Batch {
       *uploaded = true;
       return;
     }
-    if (!pref.empty()) {
-      for (int s = 0; s < B; ++s) ring_next[s] = pref.front().slot[s];
-      pref.clear();
-    }
-    fresh_slots(slot_of);
+    drop_prefetches();
+    fresh_slots(every_sequence(), slot_of);
     *uploaded = false;
   }
   int prefetch_frames(const uint8_t* const* imgs, size_t ib) {
     if (pref.size() >= 2) return fail(XIVO_ERR_STATE, "prefetch_frames: two prefetched frames are pending already (consume one with a step / visual_meas call first)");
     Prefetched p;
     p.slot.resize(B);
-    fresh_slots(p.slot);
-    if (int rc = upload_frames(imgs, p.slot, false, ib)) return rc;
+    const std::vector<int> all = every_sequence();
+    fresh_slots(all, p.slot);
+    if (int rc = upload_frames(imgs, all, p.slot, false, ib)) return rc;
     p.ptr.assign(imgs, imgs + B);
     pref.push_back(std::move(p));
     return 0;
   }
-  int upload_frames(const uint8_t* const* imgs, const std::vector<int>& slot_of, bool on_device, size_t ib) {
+  // The frames of the sequences in `seqs` (imgs[s] into ring slot slot_of[s]) go down on st_copy; the other sequences' entries are not read.
+  int upload_frames(const uint8_t* const* imgs, const std::vector<int>& seqs, const std::vector<int>& slot_of, bool on_device, size_t ib) {
     HostScope hsu("issue_upload_frames");
     const bool zero_copy = g_frame_ingest.load(std::memory_order_relaxed) == 0;
     bool gather = on_device || zero_copy;
-    for (int s = 0; s < B; ++s) {
-      ingest_off.h[s] = ((size_t)s * ring_n + slot_of[s]) * ib;
-      ingest_ptr.h[s] = imgs[s];
+    const int n = (int)seqs.size();
+    if (!n) return 0;
+    // compacted [source, ring offset] list of the present frames
+    for (int i = 0; i < n; ++i) {
+      const int s = seqs[i];
+      ingest_off.h[i] = ((size_t)s * ring_n + slot_of[s]) * ib;
+      ingest_ptr.h[i] = imgs[s];
       if (!on_device && gather) {
-        if (s == 0) host_ranges.clear();  // one real query per call keeps the cache honest if the caller re-pins / frees its pool between steps
+        if (i == 0) host_ranges.clear();  // one real query per call keeps the cache honest if the caller re-pins / frees its pool between steps
         const uint8_t* dp = mapped_host_pointer(imgs[s], ib);
         if (!dp) gather = false;
-        else ingest_ptr.h[s] = dp;
+        else ingest_ptr.h[i] = dp;
       }
     }
-    if (!on_device) Prof::get().h2d += (unsigned long long)ib * B;
+    if (!on_device) Prof::get().h2d += (unsigned long long)ib * n;
     if (gather) {
       XB_CUDA(up_blob(blobG, blobG.n, st_copy));  // [sources | ring offsets]
       // host sources: one warp per frame with four loads in flight still fills the link when several batches pull at once, and hogs it
       // less for the other batches' table fetches than wider grids do
-      if (int rc = launch_gather_frames(st_copy, ingest_ptr.d, dRing.p, 0, ingest_off.d, ib, B, on_device ? 64 : 1, on_device ? 256 : 32)) return rc;
+      if (int rc = launch_gather_frames(st_copy, ingest_ptr.d, dRing.p, 0, ingest_off.d, ib, n, on_device ? 64 : 1, on_device ? 256 : 32)) return rc;
       g_launches += 1;
     } else {
-      // copy engine: runs of sequences whose sources are evenly spaced (frames of one pinned pool) and whose ring slots agree go down as
-      // ONE pitched copy each (far fewer copy calls than one per frame)
-      int s = 0;
-      while (s < B) {
-        int e = s + 1;
-        if (e < B && slot_of[e] == slot_of[s] && imgs[e] > imgs[s]) {
-          const size_t stride = (size_t)(imgs[e] - imgs[s]);
+      // copy engine: runs of consecutive sequences whose sources are evenly spaced (frames of one pinned pool) and whose ring slots agree
+      // go down as ONE pitched copy each (far fewer copy calls than one per frame)
+      auto next_in_run = [&](int i, int j) { return seqs[j] == seqs[i] + 1 && slot_of[seqs[j]] == slot_of[seqs[i]] && imgs[seqs[j]] > imgs[seqs[i]]; };
+      int i = 0;
+      while (i < n) {
+        int e = i + 1;
+        if (e < n && next_in_run(i, e)) {
+          const size_t stride = (size_t)(imgs[seqs[e]] - imgs[seqs[i]]);
           if (stride >= ib) {
-            while (e + 1 < B && slot_of[e + 1] == slot_of[s] && imgs[e + 1] > imgs[e] && (size_t)(imgs[e + 1] - imgs[e]) == stride) ++e;
+            while (e + 1 < n && next_in_run(e, e + 1) && (size_t)(imgs[seqs[e + 1]] - imgs[seqs[e]]) == stride) ++e;
             ++e;
-            XB_CUDA(cudaMemcpy2DAsync(dRing.p + ingest_off.h[s], (size_t)ring_n * ib, imgs[s], stride, ib, (size_t)(e - s), cudaMemcpyHostToDevice, st_copy));
-            s = e;
+            XB_CUDA(cudaMemcpy2DAsync(dRing.p + ingest_off.h[i], (size_t)ring_n * ib, imgs[seqs[i]], stride, ib, (size_t)(e - i), cudaMemcpyHostToDevice,
+                                      st_copy));
+            i = e;
             continue;
           }
         }
-        XB_CUDA(cudaMemcpyAsync(dRing.p + ingest_off.h[s], imgs[s], ib, cudaMemcpyHostToDevice, st_copy));
-        ++s;
+        XB_CUDA(cudaMemcpyAsync(dRing.p + ingest_off.h[i], imgs[seqs[i]], ib, cudaMemcpyHostToDevice, st_copy));
+        ++i;
       }
     }
-    return ring_uploaded(distinct_slots(slot_of));
+    return ring_uploaded(distinct_slots(seqs, slot_of));
   }
-  static std::vector<int> distinct_slots(const std::vector<int>& slot_of) {
+  // the distinct ring slots of the frames of `seqs`
+  static std::vector<int> distinct_slots(const std::vector<int>& seqs, const std::vector<int>& slot_of) {
     std::vector<int> used;
-    for (int k : slot_of)
-      if (std::find(used.begin(), used.end(), k) == used.end()) used.push_back(k);
+    for (int s : seqs)
+      if (std::find(used.begin(), used.end(), slot_of[s]) == used.end()) used.push_back(slot_of[s]);
     return used;
   }
   // mark the uploads enqueued on st_copy for ring slot `slot` (call after the last one)
@@ -709,9 +729,9 @@ class Batch {
   }
   // the caller's frame buffers are free again once THEIR uploads have landed (the events of the ring slots they went to: a prefetched copy
   // of the next frame may already be queued behind them on st_copy and must not be waited for)
-  int ingest_done(const std::vector<int>& slot_of) {
+  int ingest_done(const std::vector<int>& seqs, const std::vector<int>& slot_of) {
     HostScope hsw("wait_ingest_done");
-    for (int k : distinct_slots(slot_of)) XB_CUDA(cudaEventSynchronize(ring_ev[k]));
+    for (int k : distinct_slots(seqs, slot_of)) XB_CUDA(cudaEventSynchronize(ring_ev[k]));
     return 0;
   }
 
@@ -719,70 +739,73 @@ class Batch {
   // with one PngFrameDesc per frame, into the pinned staging blob (in parallel on the worker pool); ONE upload on st_copy, then
   // png_inflate_kernel + png_unfilter_kernel decode straight into the ring slots of the frames and ring_ev[slot] is recorded after them,
   // so the tracker stream orders on the decode like on an upload.  The status words come back on st_copy before any message is pushed:
-  // a refused frame (host- or device-detected) leaves ring_next as the call found it and changes no sequence.  *slot_of = the slots used.
-  int decode_png_frames(const uint8_t* const* png_data, const size_t* png_bytes, int channels, std::vector<int>& slot_of) {
-    std::vector<png::Info> info(B);
-    std::vector<const char*> why(B, nullptr);
-    std::vector<size_t> zlen(B, 0);
-    std::vector<int> all(B);
-    for (int s = 0; s < B; ++s) all[s] = s;
+  // a refused frame (host- or device-detected) leaves ring_next as the call found it and changes no sequence.  Only the frames of the
+  // sequences in `seqs` are read (png_data / png_bytes / slot_of are indexed by sequence); the descriptors, the scratch space and the status
+  // words cover those frames alone.  slot_of[s] = the slot of sequence s's frame.
+  int decode_png_frames(const std::vector<int>& seqs, const uint8_t* const* png_data, const size_t* png_bytes, int channels, std::vector<int>& slot_of) {
+    const int n = (int)seqs.size();
+    if (!n) return 0;
+    std::vector<png::Info> info(n);
+    std::vector<const char*> why(n, nullptr);
+    std::vector<size_t> zlen(n, 0);
+    std::vector<int> idx(n);
+    for (int i = 0; i < n; ++i) idx[i] = i;
     {
       HostScope hp("png_parse");
-      pfor(all, [&](int s, int) {
+      pfor(idx, [&](int i, int) {
+        const int s = seqs[i];
         const char* w = "";
         size_t z = 0;
-        if (png::parse(png_data[s], png_bytes[s], info[s], &w, [&](size_t, size_t len) { z += len; })) why[s] = w;
-        zlen[s] = z;
+        if (png::parse(png_data[s], png_bytes[s], info[i], &w, [&](size_t, size_t len) { z += len; })) why[i] = w;
+        zlen[i] = z;
       });
       if (pfor_bad.load()) return fail(XIVO_ERR_STATE, "host state machine threw: " + pfor_msg);
     }
-    for (int s = 0; s < B; ++s) {
-      if (why[s]) return fail(XIVO_ERR_ARG, "png frame " + std::to_string(s) + ": " + why[s]);
-      if (channels == 1 && info[s].channels > 2)
-        return fail(XIVO_ERR_ARG, "png frame " + std::to_string(s) + ": 1-channel output needs a grey or grey + alpha PNG (colour type " +
-                                      std::to_string(info[s].color_type) + ")");
-      if (info[s].rows != info[0].rows || info[s].cols != info[0].cols)
-        return fail(XIVO_ERR_ARG, "png frame " + std::to_string(s) + " is " + std::to_string(info[s].rows) + " x " + std::to_string(info[s].cols) +
-                                      ", frame 0 is " + std::to_string(info[0].rows) + " x " + std::to_string(info[0].cols) +
-                                      ": all sequences of a batch share one geometry");
+    for (int i = 0; i < n; ++i) {
+      const std::string frame = "png frame " + std::to_string(seqs[i]);
+      if (why[i]) return fail(XIVO_ERR_ARG, frame + ": " + why[i]);
+      if (channels == 1 && info[i].channels > 2)
+        return fail(XIVO_ERR_ARG, frame + ": 1-channel output needs a grey or grey + alpha PNG (colour type " + std::to_string(info[i].color_type) + ")");
+      if (info[i].rows != info[0].rows || info[i].cols != info[0].cols)
+        return fail(XIVO_ERR_ARG, frame + " is " + std::to_string(info[i].rows) + " x " + std::to_string(info[i].cols) + ", frame " + std::to_string(seqs[0]) +
+                                      " is " + std::to_string(info[0].rows) + " x " + std::to_string(info[0].cols) + ": all sequences of a batch share one geometry");
     }
+    if (img_ready && (info[0].rows != rows || info[0].cols != cols))
+      return fail(XIVO_ERR_ARG, "png frame " + std::to_string(seqs[0]) + " is " + std::to_string(info[0].rows) + " x " + std::to_string(info[0].cols) +
+                                    ", the handle's frames are " + std::to_string(rows) + " x " + std::to_string(cols));
     if (int rc = ensure_images(info[0].rows, info[0].cols, channels)) return rc;
     const size_t ib = (size_t)rows * cols * cn;
-    const size_t table = ((size_t)B * sizeof(PngFrameDesc) + 15) & ~(size_t)15;
-    std::vector<size_t> zoff(B);
+    const size_t table = ((size_t)n * sizeof(PngFrameDesc) + 15) & ~(size_t)15;
+    std::vector<size_t> zoff(n), soff(n);
     size_t zsum = 0, scratch = 0;
-    for (int s = 0; s < B; ++s) {
-      zoff[s] = zsum;
-      zsum += zlen[s];
-      scratch += (size_t)info[s].raw_bytes();
+    for (int i = 0; i < n; ++i) {
+      zoff[i] = zsum;
+      zsum += zlen[i];
+      soff[i] = scratch;
+      scratch += (size_t)info[i].raw_bytes();
     }
     const size_t stage_bytes = table + zsum;
     // grown to 1.25 x the need: frames of one sequence compress to similar sizes
     if (png_stage.n < stage_bytes && !png_stage.alloc(stage_bytes + stage_bytes / 4)) return fail(XIVO_ERR_CUDA, "png staging allocation failed");
     if (png_scratch.n < scratch && !png_scratch.alloc(scratch + scratch / 4)) return fail(XIVO_ERR_CUDA, "png scratch allocation failed");
-    if (png_status.n < (size_t)B && !png_status.alloc(B)) return fail(XIVO_ERR_CUDA, "png status allocation failed");
+    if (png_status.n < (size_t)n && !png_status.alloc(B)) return fail(XIVO_ERR_CUDA, "png status allocation failed");
     // pending prefetches are dropped as for any call with other buffers; ring_next after that is what a refusal restores
-    if (!pref.empty()) {
-      for (int s = 0; s < B; ++s) ring_next[s] = pref.front().slot[s];
-      pref.clear();
-    }
+    drop_prefetches();
     const std::vector<int> ring_before = ring_next;
-    fresh_slots(slot_of);
+    fresh_slots(seqs, slot_of);
     PngFrameDesc* fr = reinterpret_cast<PngFrameDesc*>(png_stage.h);
     {
       HostScope hk("png_pack");
-      std::vector<size_t> soff(B);
-      size_t so = 0;
-      for (int s = 0; s < B; ++s) { soff[s] = so; so += (size_t)info[s].raw_bytes(); }
-      pfor(all, [&](int s, int) {
-        uint8_t* dst = png_stage.h + table + zoff[s];
+      pfor(idx, [&](int i, int) {
+        const int s = seqs[i];
+        uint8_t* dst = png_stage.h + table + zoff[i];
         png::Info I;
         const char* w = "";
         png::parse(png_data[s], png_bytes[s], I, &w, [&](size_t off, size_t len) { memcpy(dst, png_data[s] + off, len); dst += len; });
-        PngFrameDesc& d = fr[s];
-        d.in_off = zoff[s];
-        d.in_len = zlen[s];
-        d.scratch_off = soff[s];
+        PngFrameDesc& d = fr[i];
+        d.in_off = zoff[i];
+        d.in_len = zlen[i];
+        d.scratch_off = soff[i];
         d.out_off = ((size_t)s * ring_n + slot_of[s]) * ib;
         d.rows = I.rows;
         d.cols = I.cols;
@@ -796,17 +819,17 @@ class Batch {
     {
       HostScope hu("png_issue");
       XB_CUDA(png_stage.up(st_copy, stage_bytes));
-      if (int rc = launch_png_decode(st_copy, png_stage.d + table, png_scratch.p, dRing.p, reinterpret_cast<const PngFrameDesc*>(png_stage.d), B,
+      if (int rc = launch_png_decode(st_copy, png_stage.d + table, png_scratch.p, dRing.p, reinterpret_cast<const PngFrameDesc*>(png_stage.d), n,
                                      png_status.d))
         return rc;
-      XB_CUDA(png_status.down(st_copy, B));
-      if (int rc = ring_uploaded(distinct_slots(slot_of))) return rc;
+      XB_CUDA(png_status.down(st_copy, n));
+      if (int rc = ring_uploaded(distinct_slots(seqs, slot_of))) return rc;
     }
     { HostScope hw("wait_png"); if (int rc = wait(st_copy)) return rc; }
-    for (int s = 0; s < B; ++s)
-      if (png_status.h[s] != png::kOk) {
+    for (int i = 0; i < n; ++i)
+      if (png_status.h[i] != png::kOk) {
         ring_next = ring_before;
-        return fail(XIVO_ERR_ARG, "png frame " + std::to_string(s) + ": " + png::status_text(png_status.h[s]));
+        return fail(XIVO_ERR_ARG, "png frame " + std::to_string(seqs[i]) + ": " + png::status_text(png_status.h[i]));
       }
     return 0;
   }
@@ -1455,17 +1478,21 @@ class Batch {
   // Several messages per sequence in one call (same semantics as pushing them one by one): every
   // sequence runs ahead through its IMU messages until its heap releases a visual message; those are
   // then processed together, and the loop continues with the remaining messages.
+  // A sequence with no message (xivo_batch_feed) is not touched.
   int ingest_many(std::vector<std::vector<Msg>>& in) {
     WorkPool::get().pin_driver();
-    std::vector<int> all(B), vis;
+    std::vector<int> all(B), fed, vis;
     std::vector<size_t> pos(B, 0);
     std::vector<Msg> popped(B), vmsgs;
     std::vector<char> has(B, 0);
-    for (int b = 0; b < B; ++b) all[b] = b;
+    for (int b = 0; b < B; ++b) {
+      all[b] = b;
+      if (!in[b].empty()) fed.push_back(b);
+    }
     for (;;) {
       {
         HostScope hs("ingest_imu");
-        pfor(all, [&](int b, int) {
+        pfor(fed, [&](int b, int) {
           HostScope hx("x_ingest_imu");
           has[b] = 0;
           while (pos[b] < in[b].size()) {
@@ -1612,10 +1639,11 @@ static int visual_meas_impl(xivo_batch* b, const uint64_t* ts_ns, const uint8_t*
     in[s].type = tracker_only ? 2 : 1;
     in[s].img_slot = slot_of[s];
   }
+  const std::vector<int> all = B_.every_sequence();
   if (!uploaded)
-    if (int rc = B_.upload_frames(imgs, slot_of, on_device, ib)) return rc;
+    if (int rc = B_.upload_frames(imgs, all, slot_of, on_device, ib)) return rc;
   const int rc = B_.ingest(in);
-  const int rc2 = B_.ingest_done(slot_of);
+  const int rc2 = B_.ingest_done(all, slot_of);
   return rc ? rc : rc2;
 }
 
@@ -1635,7 +1663,7 @@ int xivo_batch_visual_meas_png(xivo_batch* b, const uint64_t* ts_ns, const uint8
   if (channels != 1 && channels != 3) return B_.fail(XIVO_ERR_ARG, "visual_meas_png: channels must be 1 or 3, got " + std::to_string(channels));
   HostScope ht("visual_meas_png_total");
   std::vector<int> slot_of(B_.B);
-  if (int rc = B_.decode_png_frames(png, png_bytes, channels, slot_of)) return rc;
+  if (int rc = B_.decode_png_frames(B_.every_sequence(), png, png_bytes, channels, slot_of)) return rc;
   std::vector<Msg> in(B_.B);
   for (int s = 0; s < B_.B; ++s) {
     in[s].ts = ts_ns[s];
@@ -1675,11 +1703,99 @@ int xivo_batch_step(xivo_batch* b, int n_imu, const uint64_t* imu_ts, const doub
       v.img_slot = slot_of[s];
     }
   }
+  const std::vector<int> all = B_.every_sequence();
   if (!uploaded)
-    if (int rc = B_.upload_frames(imgs, slot_of, on_device != 0, ib)) return rc;
+    if (int rc = B_.upload_frames(imgs, all, slot_of, on_device != 0, ib)) return rc;
   const int rc = B_.ingest_many(in);
-  const int rc2 = B_.ingest_done(slot_of);
+  const int rc2 = B_.ingest_done(all, slot_of);
   return rc ? rc : rc2;
+}
+
+// xivo_batch_feed[_png]: what is refused is refused here, before a ring slot is taken or a message pushed.
+static int feed_check(Batch& B_, const char* what, const int* n_imu, const uint64_t* imu_ts, const double* gyro, const double* accel,
+                      const uint64_t* frame_ts, bool any_frame) {
+  if (int rc = B_.refuse_if_failed(what)) return rc;
+  if (!n_imu) return B_.fail(XIVO_ERR_ARG, std::string(what) + ": null n_imu");
+  for (int s = 0; s < B_.B; ++s) {
+    if (n_imu[s] < 0) return B_.fail(XIVO_ERR_ARG, std::string(what) + ": sequence " + std::to_string(s) + ": negative n_imu (" + std::to_string(n_imu[s]) + ")");
+    if (n_imu[s] > 0 && !(imu_ts && gyro && accel))
+      return B_.fail(XIVO_ERR_ARG, std::string(what) + ": sequence " + std::to_string(s) + " has " + std::to_string(n_imu[s]) + " IMU samples but the IMU arrays are null");
+  }
+  if (any_frame && !frame_ts) return B_.fail(XIVO_ERR_ARG, std::string(what) + ": null frame_ts");
+  return 0;
+}
+// Sequence s: its n_imu[s] IMU rows (from offset sum(n_imu[0..s-1])), then its frame in ring slot slot_of[s] if it has one.
+static void feed_messages(const Batch& B_, const int* n_imu, const uint64_t* imu_ts, const double* gyro, const double* accel, const uint64_t* frame_ts,
+                          const std::vector<int>& present, const std::vector<int>& slot_of, int tracker_only, std::vector<std::vector<Msg>>& in) {
+  HostScope hm("marshal");
+  std::vector<char> has_frame(B_.B, 0);
+  for (int s : present) has_frame[s] = 1;
+  size_t o = 0;
+  for (int s = 0; s < B_.B; ++s) {
+    in[s].resize((size_t)n_imu[s] + has_frame[s]);
+    for (int k = 0; k < n_imu[s]; ++k, ++o) {
+      Msg& m = in[s][k];
+      m.ts = imu_ts[o];
+      m.type = 0;
+      memcpy(m.gyro, gyro + o * 3, 24);
+      memcpy(m.accel, accel + o * 3, 24);
+    }
+    if (has_frame[s]) {
+      Msg& v = in[s][n_imu[s]];
+      v.ts = frame_ts[s];
+      v.type = tracker_only ? 2 : 1;
+      v.img_slot = slot_of[s];
+    }
+  }
+}
+
+int xivo_batch_feed(xivo_batch* b, const int* n_imu, const uint64_t* imu_ts, const double* gyro, const double* accel, const uint64_t* frame_ts,
+                    const uint8_t* const* imgs, int rows, int cols, int channels, int on_device, int tracker_only) {
+  BATCH_BEGIN;
+  HostScope hst("feed_total");
+  std::vector<int> present;  // the sequences that get a frame
+  if (imgs)
+    for (int s = 0; s < B_.B; ++s)
+      if (imgs[s]) present.push_back(s);
+  if (int rc = feed_check(B_, "feed", n_imu, imu_ts, gyro, accel, frame_ts, !present.empty())) return rc;
+  std::vector<int> slot_of(B_.B, -1);
+  const size_t ib = (size_t)rows * cols * channels;
+  if (!present.empty()) {
+    const std::string first = std::to_string(present[0]);
+    if (rows <= 0 || cols <= 0) return B_.fail(XIVO_ERR_ARG, "feed: sequence " + first + ": bad frame geometry");
+    if (B_.img_ready && (rows != B_.rows || cols != B_.cols || channels != B_.cn))
+      return B_.fail(XIVO_ERR_ARG, "feed: sequence " + first + ": frame is " + std::to_string(rows) + " x " + std::to_string(cols) + " x " + std::to_string(channels) +
+                                       ", the handle's frames are " + std::to_string(B_.rows) + " x " + std::to_string(B_.cols) + " x " + std::to_string(B_.cn));
+    if (int rc = B_.ensure_images(rows, cols, channels)) return rc;
+    B_.drop_prefetches();
+    B_.fresh_slots(present, slot_of);
+    if (int rc = B_.upload_frames(imgs, present, slot_of, on_device != 0, ib)) return rc;
+  }
+  std::vector<std::vector<Msg>> in(B_.B);
+  feed_messages(B_, n_imu, imu_ts, gyro, accel, frame_ts, present, slot_of, tracker_only, in);
+  const int rc = B_.ingest_many(in);
+  const int rc2 = present.empty() ? 0 : B_.ingest_done(present, slot_of);
+  return rc ? rc : rc2;
+}
+
+int xivo_batch_feed_png(xivo_batch* b, const int* n_imu, const uint64_t* imu_ts, const double* gyro, const double* accel, const uint64_t* frame_ts,
+                        const uint8_t* const* png, const size_t* png_bytes, int channels, int tracker_only) {
+  BATCH_BEGIN;
+  HostScope hst("feed_png_total");
+  std::vector<int> present;
+  if (png)
+    for (int s = 0; s < B_.B; ++s)
+      if (png[s]) present.push_back(s);
+  if (int rc = feed_check(B_, "feed_png", n_imu, imu_ts, gyro, accel, frame_ts, !present.empty())) return rc;
+  std::vector<int> slot_of(B_.B, -1);
+  if (!present.empty()) {
+    if (!png_bytes) return B_.fail(XIVO_ERR_ARG, "feed_png: null png_bytes");
+    if (channels != 1 && channels != 3) return B_.fail(XIVO_ERR_ARG, "feed_png: channels must be 1 or 3, got " + std::to_string(channels));
+    if (int rc = B_.decode_png_frames(present, png, png_bytes, channels, slot_of)) return rc;
+  }
+  std::vector<std::vector<Msg>> in(B_.B);
+  feed_messages(B_, n_imu, imu_ts, gyro, accel, frame_ts, present, slot_of, tracker_only, in);
+  return B_.ingest_many(in);
 }
 
 int xivo_batch_prefetch_frames(xivo_batch* b, const uint8_t* const* imgs, int rows, int cols, int channels) {

@@ -44,6 +44,26 @@ def load_asl(image_dir: str, imu_dir: str | None = None):
     return out
 
 
+def feed_rounds(msg_lists):
+    """Schedules B message lists (the load_asl format) for pyxivo.Batch.feed / xivo_batch_feed: round r holds, per sequence, the r-th
+    piece of its list, where a piece is the IMU messages up to and including the next frame (any kind other than 'imu'), and IMU
+    messages after the last frame form a last piece.  So every round gives a sequence at most one frame, as the last message, and a
+    sequence whose list is exhausted gets an empty piece.  -> [round][sequence] lists of messages; no rounds when every list is empty."""
+    pieces = []
+    for msgs in msg_lists:
+        cur, out = [], []
+        for m in msgs:
+            cur.append(m)
+            if m[0] != "imu":
+                out.append(cur)
+                cur = []
+        if cur:
+            out.append(cur)
+        pieces.append(out)
+    n = max((len(p) for p in pieces), default=0)
+    return [[p[r] if r < len(p) else [] for p in pieces] for r in range(n)]
+
+
 def write_asl(root: str, msgs, image_writer=None):
     """Writes a message list as an ASL folder (cam0/data.csv, cam0/data/<ts>.pgm|.ppm, imu0/data.csv).  Images are stored
     as binary PGM/PPM unless `image_writer(path, array)` is given."""

@@ -90,14 +90,15 @@ class Batch:
         a = np.ascontiguousarray(np.broadcast_to(np.asarray(accel, dtype=np.float64), (self.n, 3)))
         _check(capi.lib().xivo_batch_inertial_meas(self._h, _p(ts), _p(g), _p(a)), "xivo_batch_inertial_meas")
 
-    def _check_images(self, imgs):
-        """One image per sequence, all of the same shape (rows x cols [x 1 | 3]), uint8, C-contiguous: the C side reads
+    def _check_images(self, imgs, count=None):
+        """One image per sequence (or `count` images), all of the same shape (rows x cols [x 1 | 3]), uint8, C-contiguous: the C side reads
         rows * cols * channels bytes behind every pointer."""
+        count = self.n if count is None else count
         if isinstance(imgs, np.ndarray):
-            imgs = [imgs] * self.n
+            imgs = [imgs] * count
         imgs = list(imgs)
-        if len(imgs) != self.n:
-            raise XivoError(f"expected {self.n} images (one per sequence), got {len(imgs)}")
+        if len(imgs) != count:
+            raise XivoError(f"expected {count} images (one per sequence), got {len(imgs)}")
         imgs = [np.ascontiguousarray(i, dtype=np.uint8) for i in imgs]
         shp = imgs[0].shape
         if len(shp) not in (2, 3) or (len(shp) == 3 and shp[2] not in (1, 3)):
@@ -152,6 +153,84 @@ class Batch:
         ptrs = (C.c_void_p * self.n)(*[i.ctypes.data for i in imgs])
         self._keep = imgs
         _check(capi.lib().xivo_batch_step(self._h, n_imu, _p(its), _p(g), _p(a), _p(fts), ptrs, rows, cols, ch, 0), "xivo_batch_step")
+
+    def _feed_imu(self, imu):
+        """-> n_imu (n,), imu_ts, gyro, accel: the per-sequence samples concatenated in sequence order."""
+        n_imu = np.zeros(self.n, np.int32)
+        ts, gyro, accel = [np.zeros(0, np.uint64)], [np.zeros((0, 3))], [np.zeros((0, 3))]
+        if imu is not None:
+            if len(imu) != self.n:
+                raise XivoError(f"expected {self.n} IMU entries (one per sequence, None for none), got {len(imu)}")
+            for s, e in enumerate(imu):
+                if e is None:
+                    continue
+                t = np.asarray(e[0], dtype=np.uint64).reshape(-1)
+                g = np.asarray(e[1], dtype=np.float64).reshape(-1, 3)
+                a = np.asarray(e[2], dtype=np.float64).reshape(-1, 3)
+                if len(g) != len(t) or len(a) != len(t):
+                    raise XivoError(f"sequence {s}: {len(t)} IMU stamps but {len(g)} gyro and {len(a)} accel rows")
+                n_imu[s] = len(t)
+                ts.append(t)
+                gyro.append(g)
+                accel.append(a)
+        return n_imu, np.ascontiguousarray(np.concatenate(ts)), np.ascontiguousarray(np.concatenate(gyro)), np.ascontiguousarray(np.concatenate(accel))
+
+    def _feed_frames(self, frames, what):
+        """-> frame_ts (n,), the present sequences and their payloads."""
+        fts = np.zeros(self.n, np.uint64)
+        present = []
+        if frames is not None:
+            if len(frames) != self.n:
+                raise XivoError(f"expected {self.n} {what} entries (one per sequence, None for none), got {len(frames)}")
+            for s, e in enumerate(frames):
+                if e is not None:
+                    fts[s] = int(e[0])
+                    present.append((s, e[1]))
+        return fts, present
+
+    def feed(self, imu, frames, tracker_only=False):
+        """Each sequence its own messages in one call (xivo_batch_feed): sequence s gets the IMU samples of imu[s] = (ts (k,), gyro (k, 3),
+        accel (k, 3)), in order, then the frame of frames[s] = (ts, image) if there is one.  None (for an entry or for the whole list): nothing
+        of that kind.  Images are host arrays (rows x cols [x 3], uint8) or CUDA tensors of that shape (device-resident frames); all frames of
+        one call share one geometry.  Every sequence ends bit-identical to a one-sequence handle fed the same messages one at a time."""
+        n_imu, its, g, a = self._feed_imu(imu)
+        fts, present = self._feed_frames(frames, "frame")
+        ptrs = (C.c_void_p * self.n)()
+        rows = cols = ch = on_device = 0
+        if present:
+            dev = [hasattr(i, "data_ptr") and getattr(i, "is_cuda", False) for _, i in present]
+            if any(dev) and not all(dev):
+                raise XivoError("the frames of one feed call are either all host arrays or all CUDA tensors")
+            on_device = int(dev[0])
+            if on_device:
+                shp = tuple(present[0][1].shape)
+                for s, i in present:
+                    if tuple(i.shape) != shp or not i.is_contiguous() or i.element_size() != 1:
+                        raise XivoError(f"sequence {s}: device frames must be contiguous uint8 tensors of one shape {shp}")
+                    ptrs[s] = i.data_ptr()
+                rows, cols, ch = shp[0], shp[1], (1 if len(shp) == 2 else shp[2])
+                self._keep = [i for _, i in present]
+            else:
+                imgs, rows, cols, ch = self._check_images([i for _, i in present], len(present))
+                for (s, _), i in zip(present, imgs):
+                    ptrs[s] = i.ctypes.data
+                self._keep = imgs
+        _check(capi.lib().xivo_batch_feed(self._h, _p(n_imu), _p(its), _p(g), _p(a), _p(fts), ptrs, rows, cols, ch, on_device, int(bool(tracker_only))),
+               "xivo_batch_feed")
+
+    def feed_png(self, imu, frames, channels=3, tracker_only=False):
+        """feed with the frames given as PNG file bytes, frames[s] = (ts, bytes) or None, decoded on the device as in visual_meas_png.
+        A refused or corrupt file of any sequence raises XivoError before any sequence's state changes."""
+        n_imu, its, g, a = self._feed_imu(imu)
+        fts, present = self._feed_frames(frames, "PNG frame")
+        blobs = [bytes(b) for _, b in present]
+        src = (C.c_char_p * self.n)()
+        sizes = (C.c_size_t * self.n)()
+        for (s, _), b in zip(present, blobs):
+            src[s] = b
+            sizes[s] = len(b)
+        _check(capi.lib().xivo_batch_feed_png(self._h, _p(n_imu), _p(its), _p(g), _p(a), _p(fts), src, sizes, int(channels), int(bool(tracker_only))),
+               "xivo_batch_feed_png")
 
     def visual_meas_pointcloud(self, ts_ns, ids, xp_depth, tracker_only=False):
         """ids / xp_depth: lists of per-sequence arrays, or single arrays shared by all."""
