@@ -26,7 +26,9 @@ extern "C" {
 
 typedef struct xivo_batch xivo_batch;
 
-/* CreateSystem / CreateSystemTrackerOnly (src/factory.cpp:17-122) for n_seq sequences. */
+/* CreateSystem / CreateSystemTrackerOnly (src/factory.cpp:17-122) for n_seq sequences.
+ * Unless tracker_only, an update of 2 * max_features rows must fit the update kernels' shared memory on an H100: max_features <= 77,
+ * and <= 64 with "covariance_update": "tf32x3" (no such bound under XIVO_TC_V1=1); a larger value is refused with XIVO_ERR_ARG. */
 int xivo_batch_create(xivo_ctx* ctx, const char* cfg_json, int n_seq, int max_groups, int max_features,
                       int tracker_only, xivo_batch** out);
 void xivo_batch_destroy(xivo_batch* b);

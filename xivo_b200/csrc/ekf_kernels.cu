@@ -417,12 +417,20 @@ static size_t gain_smem(int Mmax, bool sparse) {
   return s;
 }
 
+int ekf_gain_max_rows(bool sparse) {
+  int m = 0;
+  while (gain_smem(m + 1, sparse) <= kSmemOptin) ++m;
+  return m;
+}
+
 int launch_ekf_update(cudaStream_t st, EkfLayout lay, const FeatJac* jac, const int* sel, const int* nsel, const double* Rmeas,
                       double* P, double* err, double* HP, double* Kt, double* H_dense, int batch, int tensor_core, const EditOp* ops,
                       const int* ops_first, const int* nops, const TcOperands* tc, int full_j) {
   const int N = lay.N(), Mmax = 2 * lay.F;
+  XB_REQUIRE(Mmax <= ekf_gain_max_rows(true), "EKF update: 2*F too large for the shared-memory Cholesky");
+  const bool tc2 = tensor_core && tc && tc->kt32;
+  if (tc2) XB_REQUIRE(Mmax <= ekf_cov_tc2_max_rows(), "EKF update: 2*F too large for the tensor-core downdate's resident A operand");
   const size_t smem = gain_smem(Mmax, true);
-  XB_REQUIRE(smem <= 227 * 1024, "EKF update: 2*F too large for the shared-memory Cholesky");
   {  // one attribute call per size, not one per launch (every CUDA call of a driver thread contends with the other batches' drivers)
     static std::atomic<size_t> attr{0};
     if (smem > attr.load(std::memory_order_relaxed)) {
@@ -431,7 +439,6 @@ int launch_ekf_update(cudaStream_t st, EkfLayout lay, const FeatJac* jac, const 
     }
   }
   ProfRec* pi_ = Prof::get().start("ekf_gain", st);
-  const bool tc2 = tensor_core && tc && tc->kt32;
   ekf_gain_kernel<true><<<batch, GAIN_THREADS, smem, st>>>(N, lay, jac, sel, nsel, 0, nullptr, nullptr, nullptr, Rmeas, P, err, HP,
                                                           Kt, H_dense, Mmax, ops, ops_first, nops, tc2 ? tc->kt32 : nullptr, tc2 ? tc->hp32 : nullptr,
                                                           tc2 ? tc->Npad : 0, tc2 ? tc->KCmax : 0, full_j);
@@ -449,11 +456,12 @@ int launch_ekf_update(cudaStream_t st, EkfLayout lay, const FeatJac* jac, const 
 
 int launch_ekf_update_dense(cudaStream_t st, int N, int M, const double* H, const double* diagR, const double* inn, double* P,
                             double* err, double* HP, double* Kt, int batch, int tensor_core, const TcOperands* tc) {
+  XB_REQUIRE(M <= ekf_gain_max_rows(false), "EKF update: M too large for the shared-memory Cholesky");
+  const bool tc2 = tensor_core && tc && tc->kt32;
+  if (tc2) XB_REQUIRE(M <= ekf_cov_tc2_max_rows(), "EKF update: M too large for the tensor-core downdate's resident A operand");
   const size_t smem = gain_smem(M, false);
-  XB_REQUIRE(smem <= 227 * 1024, "EKF update: M too large for the shared-memory Cholesky");
   XB_CUDA(cudaFuncSetAttribute(ekf_gain_kernel<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
   EkfLayout lay{0, 0};
-  const bool tc2 = tensor_core && tc && tc->kt32;
   {
     ProfScope pg("ekf_gain", st);
     ekf_gain_kernel<false><<<batch, GAIN_THREADS, smem, st>>>(N, lay, nullptr, nullptr, nullptr, M, H, diagR, inn, nullptr, P, err,

@@ -401,9 +401,15 @@ size_t ekf_cov_tc2_smem(int KCmax) {
   return kbmax * 2 * T2_A_BLOCK + 2 * kbmax * 2 * T2_B_BLOCK + (size_t)T2_MT * (T2_NT + 1) * sizeof(float);
 }
 
+int ekf_cov_tc2_max_rows() {
+  int m = 0;
+  while (ekf_cov_tc2_smem(tc_kcmax(m + 1)) <= kSmemOptin) ++m;
+  return m;
+}
+
 int launch_ekf_cov_tc2(cudaStream_t st, int N, const int* nsel, int Mdense, const TcOperands& t, double* P, int batch) {
+  XB_REQUIRE(t.KCmax <= tc_kcmax(ekf_cov_tc2_max_rows()), "tensor-core downdate: measurement dimension too large for the resident A operand");
   const size_t smem = ekf_cov_tc2_smem(t.KCmax);
-  XB_REQUIRE(smem <= 227 * 1024, "tensor-core downdate: measurement dimension too large for the resident A operand");
   XB_REQUIRE(batch <= t.batch, "tensor-core downdate: operand buffers hold fewer filters");
   static std::atomic<size_t> attr{0};
   if (smem > attr.load(std::memory_order_relaxed)) {

@@ -337,6 +337,17 @@ class Batch {
       est.back()->compact_records = true;  // imu_cov_propagate rebuilds the intermediate Runge-Kutta stages itself
     }
     cov_tc = est[0]->c.cov_update_tf32x3 ? 1 : 0;
+    const bool tc2 = cov_tc && !(getenv("XIVO_TC_V1") && getenv("XIVO_TC_V1")[0] == '1');
+    if (!tracker_only) {  // an update of 2 * max_features rows must fit the kernels' resident shared-memory working sets (kernels.h)
+      const int gain_f = ekf_gain_max_rows(true) / 2, tc2_f = ekf_cov_tc2_max_rows() / 2;
+      if (lay.F > gain_f)
+        throw std::runtime_error("max_features = " + std::to_string(lay.F) + " exceeds " + std::to_string(gain_f) +
+                                 ", the most the gain kernel's shared-memory Cholesky holds");
+      if (tc2 && lay.F > tc2_f)
+        throw std::runtime_error("max_features = " + std::to_string(lay.F) + " exceeds " + std::to_string(tc2_f) +
+                                 ", the most the \"tf32x3\" covariance downdate holds (XIVO_TC_V1=1 selects the first tensor-core kernel, "
+                                 "which has no such limit)");
+    }
     use_1pt = est[0]->c.use_1pt_RANSAC;
     table_order.resize(B);
     maxops = 4 * (lay.F + lay.G) + 16;
@@ -364,7 +375,7 @@ class Batch {
              t.put(stg_first[h], nB); t.put(stg_n[h], nB);
              blobI_fixed = t.put(stg[h], nB * kMaxSteps);
            });
-    if (ok && cov_tc && !(getenv("XIVO_TC_V1") && getenv("XIVO_TC_V1")[0] == '1')) {
+    if (ok && tc2) {
       const size_t words = tc_operand_words(N, 2 * lay.F, B);
       ok = dKt32.alloc(words) && dHP32.alloc(words) && cudaMemset(dKt32.p, 0, words * 4) == cudaSuccess && cudaMemset(dHP32.p, 0, words * 4) == cudaSuccess &&
            tc_operands_init(&tcops, N, 2 * lay.F, B, dKt32.p, dHP32.p) == 0;

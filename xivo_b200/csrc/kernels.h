@@ -106,6 +106,14 @@ int launch_jacobian_gate(cudaStream_t st, EkfLayout lay, const CameraParams* cam
                          int batch, const EditOp* ops = nullptr /*packed edit lists applied to P first*/, const int* ops_first = nullptr /*B*/,
                          const int* nops = nullptr /*B*/, double* diag_out = nullptr /*B x N: diag(P) after the edits*/);
 
+// The update kernels keep their per-filter working set resident in shared memory, so the measurement dimension is bounded by
+// Hopper's per-block opt-in limit.  ekf_gain_max_rows: the largest M (sparse: Mmax = 2F) whose S, innovation and sparse H fit;
+// ekf_cov_tc2_max_rows: the largest Mmax whose resident A operand of the second tensor-core formulation fits.  The first tensor-core
+// formulation streams K in blocks and has no such bound.  The launchers and xivo_batch_create check the same functions.
+constexpr size_t kSmemOptin = 227 * 1024;
+int ekf_gain_max_rows(bool sparse);
+int ekf_cov_tc2_max_rows();
+
 struct TcOperands;  // TF32 operand buffers + tensor maps of the tensor-core downdate (below)
 // Stack H (FillJacobianBlock semantics) for the selected features and do the measurement update.
 //   sel: B x F indices into the feature table, nsel: B counts (M = 2*nsel)
