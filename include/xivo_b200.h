@@ -80,6 +80,12 @@ int xivo_hamming_match(xivo_ctx* ctx, const uint8_t* query, int nq, const uint8_
 int xivo_fast_detect(xivo_ctx* ctx, const uint8_t* img, int rows, int cols, int cn, int threshold, int nonmax,
                      int* kp_xy, int* kp_score, int max_kp, int* n_kp);
 
+/* cv::normalize(img, out, 0, 255, cv::NORM_MINMAX) of n frames, as the tracker runs it on every frame when tracker_cfg.normalize is
+ * set (src/tracker.cpp:343-344, :465-467).  in / out: n frames of rows x cols x cn bytes back to back (out may equal in).  The minimum
+ * and maximum of a frame are taken over all its channels together; a constant frame becomes all zeros.  Refused with XIVO_ERR_ARG
+ * before the device is touched: n < 0 or n > 65535, rows or cols < 1, cn other than 1 or 3, null arrays, more than 2^40 bytes. */
+int xivo_normalize_minmax(xivo_ctx* ctx, int n, int rows, int cols, int cn, const uint8_t* in, uint8_t* out);
+
 /* Pyramidal Lucas-Kanade; replaces cv::calcOpticalFlowPyrLK at src/tracker.cpp:526-528
  * (criteria COUNT|EPS, default minEigThreshold 1e-4, flags = OPTFLOW_USE_INITIAL_FLOW when
  * use_initial_flow).  next_pts is in/out (initial guess -> result).  Multi-channel images are

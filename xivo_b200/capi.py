@@ -123,6 +123,17 @@ class Context:
         k = min(n.value, max_kp)
         return xy[:k].copy(), sc[:k].copy(), n.value
 
+    def normalize_minmax(self, frames: np.ndarray, channels: int = 1):
+        """xivo_normalize_minmax: cv2.normalize(f, None, 0, 255, cv2.NORM_MINMAX) of each frame of an (n, rows, cols) (channels = 1) or
+        (n, rows, cols, 3) (channels = 3) uint8 array; returns a new array of the same shape."""
+        frames = np.ascontiguousarray(frames, dtype=np.uint8)
+        if frames.ndim != (3 if channels == 1 else 4) or (channels == 3 and frames.shape[3] != 3):
+            raise ValueError(f"normalize_minmax: expected (n, rows, cols{'' if channels == 1 else ', 3'}) frames, got {frames.shape}")
+        n, rows, cols = frames.shape[:3]
+        out = np.empty_like(frames)
+        _check(lib().xivo_normalize_minmax(self._h, n, rows, cols, int(channels), _p(frames), _p(out)), "xivo_normalize_minmax")
+        return out
+
     def lk_track(self, prev, nxt, prev_pts, init_pts, win=15, max_level=5, max_iter=30, eps=0.01, use_initial_flow=True, min_eig=1e-4):
         prev = np.ascontiguousarray(prev, dtype=np.uint8)
         nxt = np.ascontiguousarray(nxt, dtype=np.uint8)

@@ -196,6 +196,30 @@ int xivo_hamming_match(xivo_ctx* ctx, const uint8_t* query, int nq, const uint8_
   return XIVO_OK;
 }
 
+int xivo_normalize_minmax(xivo_ctx* ctx, int n, int rows, int cols, int cn, const uint8_t* in, uint8_t* out) {
+  // the arguments are checked before the device is touched
+  XB_REQUIRE(n >= 0 && n <= 65535 && rows > 0 && cols > 0 && (cn == 1 || cn == 3) && (n == 0 || (in && out)), "normalize_minmax: bad arguments");
+  const size_t ib = (size_t)rows * cols * cn;
+  XB_REQUIRE(n == 0 || ib <= ((size_t)1 << 40) / (size_t)n, "normalize_minmax: frames too large");
+  API_BEGIN;
+  if (n == 0) return XIVO_OK;
+  cudaStream_t st = ctx->stream;
+  // the frames lie back to back as in the estimator's frame ring: a frame of odd size starts off the 16-byte grid
+  DevBuf<uint8_t> dimg((size_t)n * ib);
+  DevBuf<uint8_t*> dptr(n);
+  DevBuf<unsigned> dpart((size_t)n * kNormMaxChunks);
+  XB_REQUIRE(dimg.ok() && dptr.ok() && dpart.ok(), "cudaMalloc failed");
+  std::vector<uint8_t*> hptr(n);
+  for (int i = 0; i < n; ++i) hptr[i] = dimg.p + (size_t)i * ib;
+  XB_CUDA(cudaMemcpyAsync(dimg.p, in, (size_t)n * ib, cudaMemcpyHostToDevice, st));
+  XB_CUDA(cudaMemcpyAsync(dptr.p, hptr.data(), sizeof(uint8_t*) * n, cudaMemcpyHostToDevice, st));
+  if (int rc = launch_normalize_minmax(st, dptr.p, ib, n, dpart.p)) return rc;
+  g_launches += 2;
+  XB_CUDA(cudaMemcpyAsync(out, dimg.p, (size_t)n * ib, cudaMemcpyDeviceToHost, st));
+  XB_CUDA(cudaStreamSynchronize(st));
+  return XIVO_OK;
+}
+
 int xivo_lk_track(xivo_ctx* ctx, const uint8_t* prev, const uint8_t* next, int rows, int cols, int cn, const float* prev_pts,
                   float* next_pts, uint8_t* status, float* err, int npts, int win, int max_level, int max_iter, double eps,
                   int use_initial_flow, double min_eig_threshold) {

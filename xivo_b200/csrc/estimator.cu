@@ -294,7 +294,8 @@ class Batch {
   struct Prefetched { std::vector<const uint8_t*> ptr; std::vector<int> slot; };
   std::deque<Prefetched> pref;  // oldest first; at most two (the frame about to be consumed and the one after it)
   View<unsigned long long> off_prev, off_cur;
-  View<const uint8_t*> frame_ptr, ingest_ptr;  // ring slot of the frame being tracked; sources of a device-resident ingest
+  View<uint8_t*> frame_ptr;                    // ring slot of the frame being tracked (written in place by the normalisation)
+  View<const uint8_t*> ingest_ptr;             // sources of a device-resident ingest
   View<unsigned long long> ingest_off;
   Mirror<unsigned char> blobG;                 // [ingest_ptr | ingest_off]: one copy per gather launch
   View<float> pts0, pts1;
@@ -873,6 +874,8 @@ class Batch {
       dev_decide = !e0.tc.do_outlier_rejection && !e0.tc.extract_descriptor && track_mask_bytes(rows, cols) <= 200 * 1024 && max_pts <= 1024 && !(hd && hd[0] == '1');
     }
     desc_on = e0.tc.extract_descriptor;
+    norm_on = e0.tc.normalize;
+    if (ok && norm_on) ok = norm_part.alloc(nB * kNormMaxChunks);
     if (ok && desc_on)
       ok = descT.alloc(npt * 32) && validT.alloc(npt) && kpxy.alloc(nk * 2) && nkps.alloc(B) && nq.alloc(B) && descK.alloc(nk * 32) && validK.alloc(nk) &&
            qdesc.alloc(npt * 32) && bestT_idx.alloc(npt) && bestT_dist.alloc(npt) && bestQ_idx.alloc(nk) && bestQ_dist.alloc(nk);
@@ -910,10 +913,10 @@ class Batch {
   }
 
   // The frame of every sequence in `act` (ring slot slots[i]) goes into the free half of the sequence's pyramid buffer: the tracker stream
-  // waits for the slots' uploads; off_cur / off_prev / frame_ptr (and the TMA image indices) of the sequences, ~0 / 0 for the others.
+  // waits for the slots' uploads; off_cur / off_prev / frame_ptr (and the TMA image indices) of the sequences, ~0 / 0 / null for the others.
   int begin_frame(const std::vector<int>& act, const std::vector<int>& slots) {
     const size_t ib = (size_t)rows * cols * cn;
-    for (int b = 0; b < B; ++b) { off_cur.h[b] = ~0ull; off_prev.h[b] = 0; npts.h[b] = 0; }
+    for (int b = 0; b < B; ++b) { off_cur.h[b] = ~0ull; off_prev.h[b] = 0; npts.h[b] = 0; frame_ptr.h[b] = nullptr; }
     std::vector<char> seen(ring_n, 0);
     for (int k : slots)
       if (!seen[k]) { seen[k] = 1; XB_CUDA(cudaStreamWaitEvent(st1, ring_ev[k], 0)); }
@@ -928,7 +931,13 @@ class Batch {
     return 0;
   }
   // The pyramid passes of the frames begun by begin_frame: every level (LK), or level 0 only (MATCH: the image FAST and BRIEF read).
+  // With tracker_cfg.normalize each of those frames is first normalised in its ring slot (frame_ptr, null for the others): the slot is
+  // the library's own copy of the frame whatever the ingest path, so the caller's memory is never written.
   int build_pyramids(bool all_levels) {
+    if (norm_on) {
+      if (int rc = launch_normalize_minmax(st1, frame_ptr.d, (size_t)rows * cols * cn, B, norm_part.p)) return rc;
+      g_launches += 2;
+    }
     if (tma_pyr) {
       std::optional<ProfScope> ps;
       if (all_levels) ps.emplace("pyrdown", st1);
@@ -1088,7 +1097,7 @@ class Batch {
       for (int b : act) {
         if (kind[b] == Estimator::kTrkFirst) det_list.push_back(b);
         else if (kind[b] == Estimator::kTrkLK) lk_list.push_back(b);
-        else off_cur.h[b] = ~0ull;
+        else { off_cur.h[b] = ~0ull; frame_ptr.h[b] = nullptr; }
       }
     }
     std::unique_ptr<HostScope> hs_issue(new HostScope("issue_tracker"));
@@ -1565,6 +1574,13 @@ class Batch {
     if (vis.empty()) return 0;
     return process_visual(vis, vmsgs);
   }
+
+ private:
+  // tracker_cfg.normalize (tracker.cpp:343-344, :465-467): cv::normalize NORM_MINMAX of every new frame in its ring slot before its first
+  // pyramid pass; norm_part holds the per-CTA partial min / max of launch_normalize_minmax.  Declared after every other member, so that
+  // the members the per-frame host phases touch keep the layout they have without the option.
+  bool norm_on = false;
+  DevBuf<unsigned> norm_part;
 };
 
 }  // namespace xb

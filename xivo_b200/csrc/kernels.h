@@ -23,6 +23,10 @@ int launch_pyrdown_tma(cudaStream_t st, const CUtensorMap& map, const int* src_i
                        const unsigned long long* seq_off, const PyrDesc& d, int lvl, int ingest, int batch);
 int launch_gather_frames(cudaStream_t st, const uint8_t* const* src, uint8_t* dst, unsigned long long stride, const unsigned long long* off,
                          size_t bytes, int batch, int max_chunks = 64, int threads = 256);
+// cv::normalize(img, img, 0, 255, NORM_MINMAX) in place on frames[z] (device array of `batch` pointers, bytes each, any alignment;
+// null = skip): two launches (minmax_partial_kernel, normalize_remap_kernel).  part: batch x kNormMaxChunks words of scratch.
+constexpr int kNormMaxChunks = 64;
+int launch_normalize_minmax(cudaStream_t st, uint8_t* const* frames, size_t bytes, int batch, unsigned* part);
 // need (device, optional): per-sequence gate written by the accept kernel; a sequence with need <= 0 is skipped
 int launch_fast_detect(cudaStream_t st, const uint8_t* img, unsigned long long img_stride, const unsigned long long* seq_off,
                        int rows, int cols, int cn, int thr, int nonmax, unsigned* kp_out, int max_kp, int* kp_count, int batch,

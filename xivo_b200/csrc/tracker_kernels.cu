@@ -60,6 +60,108 @@ int launch_gather_frames(cudaStream_t st, const uint8_t* const* src, uint8_t* ds
   return 0;
 }
 
+// ------------------------------------------------------------------------------------------
+// cv::normalize(image, img_, 0, 255, NORM_MINMAX) (tracker.cpp:343-344, :465-467), in place on one frame per sequence.
+// min / max are taken over all channels together; OpenCV then runs convertTo with
+//   scale = 255 * (max - min > DBL_EPSILON ? 1 / (max - min) : 0), shift = -min * scale   (double, rounded to float)
+//   out = saturate_u8(rint(fmaf(v, scale, shift)))
+// which is bit-exact against cv2 over every (min, max, v).  Two launches: per-CTA partial min / max, then every CTA of a frame
+// folds its frame's partials and remaps its share.  A frame starts anywhere (ring slot b * ring_n + slot of a frame of odd size):
+// the bytes before its first and after its last 16-byte boundary go through CTA 0 one per thread.
+// ------------------------------------------------------------------------------------------
+constexpr int NM_THREADS = 256;
+static int normalize_chunks(size_t bytes) {
+  const size_t per = (size_t)NM_THREADS * 16 * 4;  // four 16-byte words per thread before a CTA loops
+  return (int)std::min<size_t>(kNormMaxChunks, std::max<size_t>(1, (bytes + per - 1) / per));
+}
+// [head | 16-byte aligned body of nv words | tail] of a frame at p
+struct FrameSplit {
+  size_t head, nv, tail0;
+  __device__ FrameSplit(const uint8_t* p, size_t bytes) {
+    head = (16 - (reinterpret_cast<uintptr_t>(p) & 15)) & 15;
+    if (head > bytes) head = bytes;
+    nv = (bytes - head) >> 4;
+    tail0 = head + nv * 16;
+  }
+};
+__device__ __forceinline__ unsigned bytes_min(unsigned w) { return min(min(w & 255u, (w >> 8) & 255u), min((w >> 16) & 255u, w >> 24)); }
+__device__ __forceinline__ unsigned bytes_max(unsigned w) { return max(max(w & 255u, (w >> 8) & 255u), max((w >> 16) & 255u, w >> 24)); }
+
+__global__ void __launch_bounds__(NM_THREADS) minmax_partial_kernel(uint8_t* const* __restrict__ frames, size_t bytes, unsigned* __restrict__ part) {
+  const uint8_t* __restrict__ p = frames[blockIdx.y];
+  if (!p) return;
+  const FrameSplit s(p, bytes);
+  const uint4* __restrict__ body = reinterpret_cast<const uint4*>(p + s.head);
+  unsigned mn = 0xffffffffu, mx = 0;  // four byte lanes each
+  for (size_t i = (size_t)blockIdx.x * NM_THREADS + threadIdx.x; i < s.nv; i += (size_t)gridDim.x * NM_THREADS) {
+    const uint4 v = body[i];
+    mn = __vminu4(__vminu4(mn, v.x), __vminu4(v.y, __vminu4(v.z, v.w)));
+    mx = __vmaxu4(__vmaxu4(mx, v.x), __vmaxu4(v.y, __vmaxu4(v.z, v.w)));
+  }
+  if (blockIdx.x == 0) {
+    const size_t t = threadIdx.x;
+    if (t < s.head) { const unsigned b = p[t] * 0x01010101u; mn = __vminu4(mn, b); mx = __vmaxu4(mx, b); }
+    if (s.tail0 + t < bytes) { const unsigned b = p[s.tail0 + t] * 0x01010101u; mn = __vminu4(mn, b); mx = __vmaxu4(mx, b); }
+  }
+  unsigned lo = __reduce_min_sync(0xffffffffu, bytes_min(mn)), hi = __reduce_max_sync(0xffffffffu, bytes_max(mx));
+  __shared__ unsigned wlo[NM_THREADS / 32], whi[NM_THREADS / 32];
+  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+  if (lane == 0) { wlo[warp] = lo; whi[warp] = hi; }
+  __syncthreads();
+  if (warp == 0) {
+    lo = __reduce_min_sync(0xffffffffu, lane < NM_THREADS / 32 ? wlo[lane] : 255u);
+    hi = __reduce_max_sync(0xffffffffu, lane < NM_THREADS / 32 ? whi[lane] : 0u);
+    if (lane == 0) part[(size_t)blockIdx.y * kNormMaxChunks + blockIdx.x] = lo | hi << 8;
+  }
+}
+
+__device__ __forceinline__ unsigned remap4(unsigned w, float scale, float shift) {
+  unsigned r = 0;
+#pragma unroll
+  for (int k = 0; k < 4; ++k) {
+    const int q = __float2int_rn(__fmaf_rn((float)((w >> (8 * k)) & 255u), scale, shift));
+    r |= (unsigned)min(max(q, 0), 255) << (8 * k);
+  }
+  return r;
+}
+
+__global__ void __launch_bounds__(NM_THREADS) normalize_remap_kernel(uint8_t* const* __restrict__ frames, size_t bytes, const unsigned* __restrict__ part) {
+  uint8_t* __restrict__ p = frames[blockIdx.y];
+  if (!p) return;
+  // every warp folds the frame's gridDim.x partials itself (at most two per lane): no shared memory, no barrier
+  const unsigned* pp = part + (size_t)blockIdx.y * kNormMaxChunks;
+  const unsigned lane = threadIdx.x & 31;
+  unsigned lo = 255, hi = 0;
+  for (unsigned c = lane; c < gridDim.x; c += 32) { lo = min(lo, pp[c] & 255u); hi = max(hi, pp[c] >> 8); }
+  lo = __reduce_min_sync(0xffffffffu, lo);
+  hi = __reduce_max_sync(0xffffffffu, hi);
+  const double scale_d = 255.0 * (hi > lo ? 1.0 / (double)(hi - lo) : 0.0);  // integer min / max: max - min > DBL_EPSILON <=> max > min
+  const double shift_d = 0.0 - (double)lo * scale_d;
+  const float scale = __double2float_rn(scale_d), shift = __double2float_rn(shift_d);
+  const FrameSplit s(p, bytes);
+  uint4* __restrict__ body = reinterpret_cast<uint4*>(p + s.head);
+  for (size_t i = (size_t)blockIdx.x * NM_THREADS + threadIdx.x; i < s.nv; i += (size_t)gridDim.x * NM_THREADS) {
+    uint4 v = body[i];
+    v.x = remap4(v.x, scale, shift); v.y = remap4(v.y, scale, shift); v.z = remap4(v.z, scale, shift); v.w = remap4(v.w, scale, shift);
+    body[i] = v;
+  }
+  if (blockIdx.x == 0) {
+    const size_t t = threadIdx.x;
+    if (t < s.head) p[t] = (uint8_t)remap4(p[t], scale, shift);
+    if (s.tail0 + t < bytes) p[s.tail0 + t] = (uint8_t)remap4(p[s.tail0 + t], scale, shift);
+  }
+}
+
+int launch_normalize_minmax(cudaStream_t st, uint8_t* const* frames, size_t bytes, int batch, unsigned* part) {
+  if (batch <= 0 || bytes == 0) return 0;
+  ProfScope ps("normalize_minmax", st);
+  const dim3 grid(normalize_chunks(bytes), batch);
+  minmax_partial_kernel<<<grid, NM_THREADS, 0, st>>>(frames, bytes, part);
+  normalize_remap_kernel<<<grid, NM_THREADS, 0, st>>>(frames, bytes, part);
+  XB_CUDA(cudaGetLastError());
+  return 0;
+}
+
 constexpr int PD_TX = 32, PD_TY = 8;
 
 template <int CN>
