@@ -13,6 +13,9 @@
 // round the trajectory line of every sequence that received a frame is written to its out_state: the lines a solo run writes at
 // that sequence's frame messages.  `--batch --plan <list.txt>` stops after loading and prints one line per piece:
 // `round sequence n_imu frame_ts` (`-` for a piece without a frame).
+//   vio --batch --isolate-failures <estimator_cfg.json> <list.txt> [max_groups max_features]
+// confines a failure to its sequence (Batch::IsolateFailures): a sequence that fails is reported on stderr with its image_dir and
+// message, its out_state ends at its last frame before the failure, the other sequences run to their end, and the exit status is 4.
 // Build: g++ -std=c++17 -O2 -I include examples/vio.cpp -o vio -L xivo_b200 -lxivo_b200 -Wl,-rpath,$PWD/xivo_b200
 #include <cstdio>
 #include <cstring>
@@ -56,10 +59,15 @@ static std::vector<SeqLine> read_list(const std::string& path) {
   return out;
 }
 
-static int run_batch(int argc, char** argv) {
+static int run_batch(int argc, char** argv_in) {
+  std::vector<char*> args(argv_in, argv_in + argc);
+  const bool isolate = argc >= 3 && !std::strcmp(args[2], "--isolate-failures");
+  if (isolate) args.erase(args.begin() + 2);
+  argc = (int)args.size();
+  char** argv = args.data();
   const bool plan = argc >= 4 && !std::strcmp(argv[2], "--plan");
   if (argc < 4) {
-    std::fprintf(stderr, "usage: %s --batch <estimator_cfg.json> <list.txt> [max_groups max_features] | --batch --plan <list.txt>\n", argv[0]);
+    std::fprintf(stderr, "usage: %s --batch [--isolate-failures] <estimator_cfg.json> <list.txt> [max_groups max_features] | --batch --plan <list.txt>\n", argv[0]);
     return 1;
   }
   const std::vector<SeqLine> list = read_list(argv[3]);
@@ -89,6 +97,17 @@ static int run_batch(int argc, char** argv) {
   }
   const int G = argc > 5 ? std::atoi(argv[4]) : 15, F = argc > 5 ? std::atoi(argv[5]) : 30;
   xivo::Batch batch(read_text(argv[2]), B, G, F);
+  if (isolate) batch.IsolateFailures(true);
+  std::vector<char> failed(B, 0);
+  // an isolating handle: report the sequences that failed during a call; their trajectories end here
+  auto report = [&](bool ok) {
+    if (ok) return;
+    for (const auto& kv : batch.Failed())
+      if (!failed[kv.first]) {
+        failed[kv.first] = 1;
+        std::fprintf(stderr, "sequence %d (%s) failed: error %d: %s\n", kv.first, list[kv.first].image_dir.c_str(), kv.second.code, kv.second.msg.c_str());
+      }
+  };
   std::vector<std::ofstream> out(B);
   for (int s = 0; s < B; ++s) {
     if (!list[s].cfg.empty()) {
@@ -127,7 +146,7 @@ static int run_batch(int argc, char** argv) {
         in.image = xivo::ImageView{pixels[s].data.data(), pixels[s].rows, pixels[s].cols, pixels[s].channels};
       }
     }
-    if (any_pnm || !any_png) batch.Feed(pnm);
+    if (any_pnm || !any_png) report(batch.Feed(pnm));
     if (any_png) {
       if (!any_pnm)  // the round's only call carries the IMU samples
         for (int s = 0; s < B; ++s) {
@@ -135,18 +154,25 @@ static int run_batch(int argc, char** argv) {
           png[s].gyro.swap(pnm[s].gyro);
           png[s].accel.swap(pnm[s].accel);
         }
-      batch.FeedPng(png);
+      report(batch.FeedPng(png));
     }
     for (int s = 0; s < B; ++s)
-      if (frame_of(s, r)) {
+      if (frame_of(s, r) && !failed[s]) {
         const auto g = batch.gsb(s);
         out[s] << xivo::TrajectoryLine(batch.ts(s).count(), g.data()) << "\n";
       }
   }
-  for (int s = 0; s < B; ++s)
+  int n_failed = 0;
+  for (int s = 0; s < B; ++s) {
+    if (failed[s]) {
+      std::printf("sequence %d: %d messages, failed\n", s, loaders[s]->size());
+      ++n_failed;
+      continue;
+    }
     std::printf("sequence %d: %d messages, %d in-state features, %d groups\n", s, loaders[s]->size(), batch.num_instate_features(s),
                 batch.num_instate_groups(s));
-  return 0;
+  }
+  return n_failed ? 4 : 0;
 }
 
 int main(int argc, char** argv) {

@@ -29,6 +29,9 @@ extern "C" {
 #define XIVO_ERR_CUDA (-2)  /* CUDA runtime failure, incl. "no device" */
 #define XIVO_ERR_STATE (-3) /* call not valid in the current state (reference: throw std::invalid_argument) */
 #define XIVO_ERR_SLOTS (-4) /* out of group/feature slots (reference: throw std::runtime_error, estimator.cpp:821,844) */
+/* Not an error: a message call of a batch handle that isolates failures (xivo_batch_isolate_failures) returns it when one or more of
+ * its sequences failed during the call and every other sequence finished the call normally. */
+#define XIVO_SEQ_FAILED 1
 
 typedef struct xivo_ctx xivo_ctx; /* one CUDA device + stream + scratch */
 

@@ -17,6 +17,7 @@
 #include <cstdint>
 #include <fstream>
 #include <iterator>
+#include <map>
 #include <memory>
 #include <stdexcept>
 #include <string>
@@ -315,7 +316,9 @@ class Estimator {
 
 // One handle of n independent sequences, each fed its own messages per call (xivo_batch_feed / xivo_batch_feed_png): recorded
 // sequences with different start times, lengths, IMU rates and dropped frames run side by side, every one of them bit-identical to an
-// Estimator fed the same messages one at a time.  Getters take the sequence index.
+// Estimator fed the same messages one at a time.  Getters take the sequence index.  With IsolateFailures(true) a failed sequence does
+// not end the run: Feed / FeedPng return false when sequences failed during the call, Failed() lists them with their messages, and
+// their getters throw until ResetSequence brings them back.
 class Batch {
  public:
   // What one sequence receives in one Feed / FeedPng call: its IMU samples in order, then at most one frame.
@@ -345,8 +348,29 @@ class Batch {
   Batch& operator=(const Batch&) = delete;
   int size() const { return n_; }
 
-  // in[s] for every sequence s; the frames are image views of one geometry
-  void Feed(const std::vector<Input>& in, bool tracker_only = false) {
+  // Failure isolation (xivo_batch_isolate_failures); turning it off is refused while a sequence is failed
+  void IsolateFailures(bool on) { check(xivo_batch_isolate_failures(b_, on ? 1 : 0)); }
+  struct Status { int code = 0; std::string msg; };
+  // {0, ""} while sequence `seq` runs, else its error code and message
+  Status SequenceStatus(int seq) const {
+    Status st;
+    char buf[1024];
+    check(xivo_batch_sequence_status(b_, seq, &st.code, buf, sizeof(buf)));
+    if (st.code) st.msg = buf;
+    return st;
+  }
+  // every failed sequence with its status
+  std::map<int, Status> Failed() const {
+    std::map<int, Status> out;
+    for (int s = 0; s < n_; ++s) {
+      Status st = SequenceStatus(s);
+      if (st.code) out[s] = st;
+    }
+    return out;
+  }
+
+  // in[s] for every sequence s; the frames are image views of one geometry.  false: sequences failed during the call (isolating handle)
+  bool Feed(const std::vector<Input>& in, bool tracker_only = false) {
     Flat f = flatten(in);
     std::vector<const uint8_t*> imgs(n_, nullptr);
     int rows = 0, cols = 0, ch = 0;
@@ -355,18 +379,18 @@ class Batch {
         imgs[s] = in[s].image.data;
         rows = in[s].image.rows; cols = in[s].image.cols; ch = in[s].image.channels;
       }
-    check(xivo_batch_feed(b_, f.n_imu.data(), f.ts.data(), f.gyro.data(), f.accel.data(), f.frame_ts.data(), imgs.data(), rows, cols, ch, 0,
-                          tracker_only ? 1 : 0));
+    return message(xivo_batch_feed(b_, f.n_imu.data(), f.ts.data(), f.gyro.data(), f.accel.data(), f.frame_ts.data(), imgs.data(), rows, cols, ch, 0,
+                                   tracker_only ? 1 : 0));
   }
   // the same with PNG frames (Input::png), decoded on the device like cv::imread (channels = 3: BGR)
-  void FeedPng(const std::vector<Input>& in, int channels = 3, bool tracker_only = false) {
+  bool FeedPng(const std::vector<Input>& in, int channels = 3, bool tracker_only = false) {
     Flat f = flatten(in);
     std::vector<const uint8_t*> png(n_, nullptr);
     std::vector<size_t> bytes(n_, 0);
     for (int s = 0; s < n_; ++s)
       if (in[s].has_frame) { png[s] = in[s].png.data(); bytes[s] = in[s].png.size(); }
-    check(xivo_batch_feed_png(b_, f.n_imu.data(), f.ts.data(), f.gyro.data(), f.accel.data(), f.frame_ts.data(), png.data(), bytes.data(), channels,
-                              tracker_only ? 1 : 0));
+    return message(xivo_batch_feed_png(b_, f.n_imu.data(), f.ts.data(), f.gyro.data(), f.accel.data(), f.frame_ts.data(), png.data(), bytes.data(),
+                                       channels, tracker_only ? 1 : 0));
   }
   // sequence `seq` starts over, with the handle's config (cfg_json empty) or a compatible one of its own (xivo_batch_reset_sequence)
   void ResetSequence(int seq, const std::string& cfg_json = std::string()) {
@@ -402,6 +426,11 @@ class Batch {
   }
   void check(int rc) const {
     if (rc) throw Error(rc, xivo_last_error());
+  }
+  bool message(int rc) const {
+    if (rc == XIVO_SEQ_FAILED) return false;
+    check(rc);
+    return true;
   }
   std::array<int, XIVO_NUM_COUNTERS> counters(int seq) const {
     std::array<int, XIVO_NUM_COUNTERS> c;

@@ -186,9 +186,30 @@ int xivo_init_with_sim_depths(xivo_batch* b); /* Estimator::InitWithSimDepths; a
  * Returns XIVO_ERR_ARG for a NULL handle, `seq` out of range, a config that does not parse or that
  * differs in a batch-wide setting (xivo_last_error names the first such key); XIVO_ERR_STATE once an
  * earlier call on the handle failed (such a call stops mid-frame for every sequence).  A refused
- * call changes nothing. */
+ * call changes nothing.  On a handle that isolates failures only a handle-wide failure refuses it:
+ * a failed sequence is reset like any other and runs again.
+ */
 int xivo_batch_reset_sequence(xivo_batch* b, int seq, const char* cfg_json);
 const char* xivo_batch_error(xivo_batch* b, int seq);
+
+/* Failure isolation, off by default.  Off: the first error of any sequence ends the call for every sequence mid-frame and every later
+ * call on the handle is refused.  On: a failure of one sequence is confined to that sequence --
+ *   - what counts as its failure: its estimator's sticky error (out of feature or group slots, non-finite Mahalanobis distances, an
+ *     innovation covariance that is not positive definite, a message of the wrong kind), an exception thrown by its host state machine,
+ *     or one of its per-sequence capacities exceeded (its track list over the tracker's point table, its sub-filter list, its share of
+ *     the covariance edit list);
+ *   - in the call where it fails, the sequence leaves every later phase of the frame, and the call returns XIVO_SEQ_FAILED when every
+ *     other sequence finished it normally;
+ *   - afterwards its messages are dropped by every message call (not queued, no ring slot, its PNG not parsed), its state getters
+ *     return XIVO_ERR_STATE with its message, and every other sequence continues bit-identically to a run without it;
+ *   - xivo_batch_reset_sequence brings it back, bit-identical from then on to sequence 0 of a new one-sequence handle.
+ * Handle-wide failures (CUDA errors, overflow of a buffer the sequences share, an exception while packing PNG frames) still fail the
+ * handle as a whole: the call returns the error and later calls, reset included, are refused with XIVO_ERR_STATE.
+ * Refused with XIVO_ERR_STATE on a handle that has failed as a whole, and turning isolation off while a sequence is failed. */
+int xivo_batch_isolate_failures(xivo_batch* b, int on);
+/* *code = 0 for a running sequence, else its error code; msg (msg_cap bytes, NUL-terminated, may be NULL) its message.
+ * XIVO_ERR_ARG for a NULL handle or code, or `seq` out of range. */
+int xivo_batch_sequence_status(const xivo_batch* b, int seq, int* code, char* msg, int msg_cap);
 
 #ifdef __cplusplus
 }

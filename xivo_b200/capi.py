@@ -19,6 +19,10 @@ class XivoError(RuntimeError):
     pass
 
 
+XIVO_ERR_ARG, XIVO_ERR_CUDA, XIVO_ERR_STATE, XIVO_ERR_SLOTS = -1, -2, -3, -4
+XIVO_SEQ_FAILED = 1  # a message call of a failure-isolating batch handle: sequences failed during it, the others finished it normally
+
+
 _lib = None
 
 
@@ -35,6 +39,8 @@ def lib() -> C.CDLL:
         _lib.xivo_last_error.restype = C.c_char_p
         _lib.xivo_launch_count.restype = C.c_ulonglong
         _lib.xivo_pyramid_layout.restype = C.c_ulonglong
+        _lib.xivo_batch_isolate_failures.argtypes = [C.c_void_p, C.c_int]
+        _lib.xivo_batch_sequence_status.argtypes = [C.c_void_p, C.c_int, C.POINTER(C.c_int), C.c_char_p, C.c_int]
     return _lib
 
 

@@ -214,26 +214,109 @@ class Batch {
   // (workpool.h).  CUDA calls stay on the calling thread.
   // An exception thrown by the host state machine (std::out_of_range of a container lookup, std::bad_alloc) must neither reach a
   // worker thread's top frame (std::terminate) nor unwind the publishing frame while workers still hold the job: it is caught per
-  // item, recorded, and reported by the next first_error() as a sticky batch error.
+  // item, recorded, and reported by the next first_error() as a sticky batch error.  On an isolating handle it is a failure of the
+  // item's sequence instead (owner(i): idx[i] where the items are sequences, the caller's mapping where they are positions in a list
+  // of sequences, -1 where an item belongs to no one sequence and its failure stays the handle's).
   std::atomic<int> pfor_bad{0};
   std::mutex pfor_mu;
   std::string pfor_msg;
-  void pfor_record(const char* what) {
+  void pfor_record(int seq, const char* what) {
+    if (isolate && seq >= 0) {  // only the item of this sequence writes its estimator
+      fail_sequence(seq, XIVO_ERR_STATE, std::string("host state machine threw: ") + what);
+      return;
+    }
     std::lock_guard<std::mutex> lk(pfor_mu);
     if (!pfor_bad.load()) { pfor_msg = what; pfor_bad.store(1); }
   }
-  template <typename Fn>
-  void pfor(const std::vector<int>& idx, Fn fn) {
+  template <typename Fn, typename Owner>
+  void pfor(const std::vector<int>& idx, Fn fn, Owner owner) {
     WorkPool::get().pfor((int)idx.size(), [&](int i) {
       try { fn(idx[i], i); }
-      catch (const std::exception& ex) { pfor_record(ex.what()); }
-      catch (...) { pfor_record("unknown exception"); }
+      catch (const std::exception& ex) { pfor_record(owner(i), ex.what()); }
+      catch (...) { pfor_record(owner(i), "unknown exception"); }
     });
+  }
+  template <typename Fn>
+  void pfor(const std::vector<int>& idx, Fn fn) {
+    pfor(idx, fn, [&](int i) { return idx[i]; });
   }
   int first_error(const std::vector<int>& idx) {
     if (pfor_bad.load()) return fail(XIVO_ERR_STATE, "host state machine threw: " + pfor_msg);
     for (int b : idx)
       if (est[b]->error) return fail(est[b]->error, est[b]->error_msg);
+    return 0;
+  }
+
+  // ---- failure isolation (xivo_batch_isolate_failures) -------------------------------------
+  // Off: the first error of any sequence ends the call mid-frame for every sequence, and the handle refuses what follows.  On: a
+  // sequence's own failure (its estimator's sticky error, an exception of one of its pool items, one of its per-sequence capacities)
+  // takes that sequence out of the rest of the frame and out of every later call until it is reset; only a handle-wide failure (CUDA,
+  // a shared buffer's capacity) fails the handle (dead).
+  bool isolate = false;
+  int dead = 0;
+  std::string dead_msg;
+  void fail_sequence(int b, int code, const std::string& m) {
+    Estimator& e = *est[b];
+    if (e.error) return;
+    e.error = code;
+    e.error_msg = m;
+  }
+  bool seq_failed(int b) const { return isolate && est[b]->error != 0; }
+  int n_failed() const {
+    int n = 0;
+    for (int b = 0; b < B; ++b) n += est[b]->error != 0;
+    return n;
+  }
+  // the sequences whose messages a call takes: every one, except the failed ones of an isolating handle
+  std::vector<int> live_sequences() const {
+    std::vector<int> v;
+    for (int b = 0; b < B; ++b)
+      if (!seq_failed(b)) v.push_back(b);
+    return v;
+  }
+  // Every per-sequence entry that a kernel of the rest of this frame reads is zeroed for sequence b (counts, packed-list extents,
+  // tracker kinds, pyramid and FAST selectors), so no launch reads its stale entries; the other sequences' offsets stay where they are.
+  // Called only while no upload of these host mirrors is in flight (right after a host phase, which follows a wait).
+  void quiesce(int b) {
+    nfeat.h[b] = 0; nopsJ.h[b] = 0; firstJ.h[b] = 0;
+    nsel.h[b] = 0; nopsU.h[b] = 0; firstU.h[b] = 0;
+    if (!img_ready) return;
+    npts.h[b] = 0; tkind.h[b] = 0; tneed.h[b] = 0; tnnew.h[b] = 0;
+    off_cur.h[b] = ~0ull; fast_off.h[b] = ~0ull; frame_ptr.h[b] = nullptr;
+    if (desc_on) { nkps.h[b] = 0; nq.h[b] = 0; }
+  }
+  // Isolating handle: the failed sequences leave `list` and are quiesced.  No-op otherwise.
+  void prune(std::vector<int>& list) {
+    if (!isolate) return;
+    size_t k = 0;
+    for (int b : list) {
+      if (est[b]->error) quiesce(b);
+      else list[k++] = b;
+    }
+    list.resize(k);
+  }
+  // Where a host phase of the frame ends: first_error without isolation, prune with it (a handle-wide pool failure still ends the call).
+  int settle(std::vector<int>& list) {
+    if (!isolate) return first_error(list);
+    prune(list);
+    return pool_error();
+  }
+  int pool_error() { return pfor_bad.load() ? fail(XIVO_ERR_STATE, "host state machine threw: " + pfor_msg) : 0; }
+  // A message call of an isolating handle: refused once the handle has failed; afterwards a handle-wide failure (rc < 0) fails it, and
+  // XIVO_SEQ_FAILED reports sequences that failed during the call.  Without isolation rc passes through.
+  int begin_call(const char* what) { return isolate ? refuse_if_failed(what) : 0; }
+  int end_call(int rc, int failed_before) {
+    if (!isolate) return rc;
+    if (rc < 0) {
+      if (!dead) { dead = rc; dead_msg = xivo_last_error(); }
+      return rc;
+    }
+    return n_failed() > failed_before ? XIVO_SEQ_FAILED : rc;
+  }
+  int set_isolation(bool on) {
+    if (int rc = refuse_if_failed("isolate_failures")) return rc;
+    if (!on && n_failed()) return fail(XIVO_ERR_STATE, "isolate_failures: a sequence has failed; reset it before turning isolation off");
+    isolate = on;
     return 0;
   }
   xivo_ctx* ctx;
@@ -456,9 +539,14 @@ class Batch {
     set_error("%s", m.c_str());
     return code;
   }
-  // XIVO_ERR_STATE once an earlier call on the handle failed: such a call stops mid-frame for every sequence
+  // XIVO_ERR_STATE once an earlier call on the handle failed: such a call stops mid-frame for every sequence.  On an isolating handle
+  // only a handle-wide failure counts: a failed sequence is that sequence's matter.
   int refuse_if_failed(const char* what) {
     if (pfor_bad.load()) return fail(XIVO_ERR_STATE, std::string(what) + ": an earlier call on this handle failed (" + pfor_msg + "); the handle cannot continue");
+    if (isolate) {
+      if (dead) return fail(XIVO_ERR_STATE, std::string(what) + ": an earlier call on this handle failed (" + dead_msg + "); the handle cannot continue");
+      return 0;
+    }
     for (int b = 0; b < B; ++b)
       if (est[b]->error)
         return fail(XIVO_ERR_STATE, std::string(what) + ": an earlier call on this handle failed (sequence " + std::to_string(b) + ": " + est[b]->error_msg +
@@ -487,7 +575,11 @@ class Batch {
     int n = 0;
     for (int b : act) {
       auto& e = est[b]->edits;
-      if ((int)e.size() > maxops) return fail(XIVO_ERR_STATE, "covariance edit list overflow");
+      if ((int)e.size() > maxops) {  // one sequence's share of the packed list
+        if (!isolate) return fail(XIVO_ERR_STATE, "covariance edit list overflow");
+        fail_sequence(b, XIVO_ERR_STATE, "covariance edit list overflow");
+        continue;
+      }
       first.h[b] = n;
       nops.h[b] = (int)e.size();
       for (size_t i = 0; i < e.size(); ++i) ops.h[(size_t)n + i] = e[i];
@@ -651,7 +743,8 @@ class Batch {
   // Ring slots of the frame about to be ingested.  If the oldest pending xivo_batch_prefetch_frames call brought exactly these host buffers,
   // their upload is already enqueued (*uploaded = true) and its slots are taken over; otherwise every pending prefetch is abandoned and its
   // slots are handed out again (st_copy is in order: the new upload lands after the abandoned ones).
-  void take_slots(const uint8_t* const* imgs, bool on_device, std::vector<int>& slot_of, bool* uploaded) {
+  // Fresh slots go to the sequences in `seqs` only (a failed sequence of an isolating handle takes none; its prefetched copy is ignored).
+  void take_slots(const uint8_t* const* imgs, bool on_device, const std::vector<int>& seqs, std::vector<int>& slot_of, bool* uploaded) {
     bool match = !pref.empty() && !on_device;
     if (match)
       for (int s = 0; s < B; ++s)
@@ -663,7 +756,7 @@ class Batch {
       return;
     }
     drop_prefetches();
-    fresh_slots(every_sequence(), slot_of);
+    fresh_slots(seqs, slot_of);
     *uploaded = false;
   }
   int prefetch_frames(const uint8_t* const* imgs, size_t ib) {
@@ -770,7 +863,7 @@ class Batch {
         size_t z = 0;
         if (png::parse(png_data[s], png_bytes[s], info[i], &w, [&](size_t, size_t len) { z += len; })) why[i] = w;
         zlen[i] = z;
-      });
+      }, [](int) { return -1; });  // the frames go down in one shared decode launch: a failure here is the handle's
       if (pfor_bad.load()) return fail(XIVO_ERR_STATE, "host state machine threw: " + pfor_msg);
     }
     for (int i = 0; i < n; ++i) {
@@ -825,7 +918,7 @@ class Batch {
         d.channels = I.channels;
         d.bps = I.bit_depth / 8;
         d.oc = channels;
-      });
+      }, [](int) { return -1; });
       if (pfor_bad.load()) return fail(XIVO_ERR_STATE, "host state machine threw: " + pfor_msg);
     }
     {
@@ -999,7 +1092,12 @@ class Batch {
       const int n = nkps.h[b];
       if (n) XB_CUDA(cudaMemcpyAsync(kpxy.d + (size_t)b * max_kp * 2, kpxy.h + (size_t)b * max_kp * 2, sizeof(float) * 2 * n, cudaMemcpyHostToDevice, st));
       const std::vector<Feature*>& qf = est[b]->query_feats;
-      if ((int)qf.size() > max_pts) return fail(XIVO_ERR_STATE, "descriptor matcher: more query features than max_pts");
+      if ((int)qf.size() > max_pts) {  // one sequence's share of the query table
+        if (!isolate) return fail(XIVO_ERR_STATE, "descriptor matcher: more query features than max_pts");
+        fail_sequence(b, XIVO_ERR_STATE, "descriptor matcher: more query features than max_pts");
+        nkps.h[b] = 0;  // BRIEF and both nearest-neighbour passes skip it (the callers prune it after this phase)
+        continue;
+      }
       nq.h[b] = n ? (int)qf.size() : 0;
       for (int j = 0; j < nq.h[b]; ++j) memcpy(qdesc.h + ((size_t)b * max_pts + j) * 32, qf[j]->descriptor, 32);
       if (nq.h[b]) {
@@ -1079,9 +1177,9 @@ class Batch {
 
   // Tracker::UpdateLK (tracker.cpp:463-629) for the sequences in `act` whose message holds ring slot slots[i]; the decisions are the
   // estimators' (tracker_host.cpp.inc) or, without descriptors and homography rejection, the device's (tracker_decide_on_device).
-  int tracker_update_lk(const std::vector<int>& act, const std::vector<int>& slots) {
+  int tracker_update_lk(const std::vector<int>& act_in, const std::vector<int>& slots) {
     cudaStream_t st = st1;
-    std::vector<int> lk_list, det_list, kind(B, 0);
+    std::vector<int> act = act_in, lk_list, det_list, kind(B, 0);
     {
       HostScope hs("tracker_prepare");
       if (int rc = begin_frame(act, slots)) return rc;
@@ -1090,10 +1188,14 @@ class Batch {
         HostScope hx("x_trk_prepare");
         Estimator& e = *est[b];
         kind[b] = e.tracker_lk_begin(pts0.h + (size_t)b * max_pts * 2, pts1.h + (size_t)b * max_pts * 2, max_pts);
-        if (kind[b] == Estimator::kTrkOverflow) overflow = 1;
+        if (kind[b] == Estimator::kTrkOverflow) {  // one sequence's track list
+          if (isolate) fail_sequence(b, XIVO_ERR_STATE, "tracker feature list exceeds max_pts");
+          else overflow = 1;
+        }
         if (kind[b] == Estimator::kTrkLK) npts.h[b] = (int)e.tracks.size();
       });
       if (overflow) return fail(XIVO_ERR_STATE, "tracker feature list exceeds max_pts");
+      prune(act);
       for (int b : act) {
         if (kind[b] == Estimator::kTrkFirst) det_list.push_back(b);
         else if (kind[b] == Estimator::kTrkLK) lk_list.push_back(b);
@@ -1140,6 +1242,7 @@ class Batch {
         const size_t r = (size_t)b * max_pts;
         est[b]->tracker_lk_accept(pts0.h + 2 * r, pts1.h + 2 * r, lkst.h + r, desc_on ? descT.h + 32 * r : nullptr, desc_on ? validT.h + r : nullptr);
       });
+      prune(lk_list);
       for (int b : lk_list)
         if (est[b]->detect_budget > 0) det_list.push_back(b);
     }
@@ -1154,7 +1257,9 @@ class Batch {
         pfor(det_list, [&](int b, int) {
           nkps.h[b] = est[b]->tracker_order_keypoints(kp.h + (size_t)b * max_kp, std::min(kpcount.h[b], max_kp), true, kpxy.h + (size_t)b * max_kp * 2);
         });
+        prune(det_list);
         if (int rc = describe_and_match(det_list, off_prev.d)) return rc;
+        prune(det_list);
         HostScope hs("tracker_select");
         pfor(det_list, [&](int b, int) {
           std::vector<std::array<int, 3>> m;
@@ -1176,8 +1281,9 @@ class Batch {
 
   // Tracker::UpdateMatch (tracker.cpp:341-460): detect without a mask, describe, cross-checked nearest-neighbour matching of the existing
   // features' descriptors against the new keypoints (device); the decisions are the estimators' (tracker_host.cpp.inc).
-  int tracker_update_match(const std::vector<int>& act, const std::vector<int>& slots) {
+  int tracker_update_match(const std::vector<int>& act_in, const std::vector<int>& slots) {
     cudaStream_t st = st1;
+    std::vector<int> act = act_in;
     if (int rc = begin_frame(act, slots)) return rc;
     XB_CUDA(off_cur.up(st)); XB_CUDA(frame_ptr.up(st));
     if (tma_pyr) { XB_CUDA(ring_img.up(st)); XB_CUDA(pyr_img.up(st)); }
@@ -1187,10 +1293,15 @@ class Batch {
     pfor(act, [&](int b, int) {
       Estimator& e = *est[b];
       nkps.h[b] = e.tracker_match_begin(kp.h + (size_t)b * max_kp, std::min(kpcount.h[b], max_kp), kpxy.h + (size_t)b * max_kp * 2);
-      if ((int)e.query_feats.size() > max_pts) overflow = 1;
+      if ((int)e.query_feats.size() > max_pts) {  // one sequence's track list
+        if (isolate) fail_sequence(b, XIVO_ERR_STATE, "tracker feature list exceeds max_pts");
+        else overflow = 1;
+      }
     });
     if (overflow) return fail(XIVO_ERR_STATE, "tracker feature list exceeds max_pts");
+    prune(act);
     if (int rc = describe_and_match(act, off_cur.d)) return rc;
+    prune(act);
     pfor(act, [&](int b, int) {
       std::vector<std::array<int, 3>> m;
       matches_of(b, &m);
@@ -1204,7 +1315,7 @@ class Batch {
   // Jacobians), temporary update with the low-innovation rows of J() on the covariance with the high-innovation rows zeroed, Jacobians +
   // Mahalanobis distances of the in-state features at the temporarily absorbed motion state, restore.  Sequences that do not need it
   // take part with empty tables.
-  int ransac_phases(const std::vector<int>& full) {
+  int ransac_phases(std::vector<int>& full) {
     cudaStream_t st = st2;
     HostScope hs("ransac_phases");
     std::vector<int> act;
@@ -1244,7 +1355,8 @@ class Batch {
       double* Xh = X.h + (size_t)b * kPoseDoubles;
       memcpy(Xh, e.X.Rsb.m, 72); memcpy(Xh + 9, e.X.Tsb.v, 24); memcpy(Xh + 12, e.X.Rbc.m, 72); memcpy(Xh + 21, e.X.Tbc.v, 24);
     }
-    if (int rc = first_error(full)) return rc;
+    if (int rc = settle(full)) return rc;
+    prune(act);
     // ---- phase 2: Jacobians and r' (J P J' + R)^-1 r at the temporary state (features and groups did not move: their tables are still on the device)
     std::vector<int> nfeat_saved(B);
     for (int b = 0; b < B; ++b) { nfeat_saved[b] = nfeat.h[b]; nfeat.h[b] = 0; nopsJ.h[b] = 0; firstJ.h[b] = 0; }
@@ -1260,7 +1372,8 @@ class Batch {
       XB_CUDA(cudaMemcpyAsync(dP.p + (size_t)b * N * N, dP0.p + (size_t)b * N * N, sizeof(double) * N * N, cudaMemcpyDeviceToDevice, st));
     if (int rc = wait(st)) return rc;
     for (int b : act) est[b]->ransac_finish(mh.h + (size_t)b * lay.F, table_order[b]);
-    if (int rc = first_error(full)) return rc;
+    if (int rc = settle(full)) return rc;
+    prune(act);
     // ---- phase 3: the survivors' Jacobians at the restored state (update.cpp:381-385), from their CURRENT owner and local state
     for (int b : act) {
       Estimator& e = *est[b];
@@ -1280,7 +1393,7 @@ class Batch {
                                       nullptr))
       return rc;
     g_launches += 1;
-    for (int b = 0; b < B; ++b) nfeat.h[b] = nfeat_saved[b];
+    for (int b = 0; b < B; ++b) nfeat.h[b] = seq_failed(b) ? 0 : nfeat_saved[b];
     return 0;
   }
 
@@ -1298,9 +1411,10 @@ class Batch {
         Msg& m = msgs[i];
         if (!e.visual_begin(m.ts, m.type) || e.error) return;
         proceed[i] = 1;
-      });
+      }, [&](int i) { return act_in[i]; });
     }
-    if (int rc = first_error(act_in)) return rc;
+    // isolating: a sequence that failed here has proceed = 0 already
+    if (int rc = isolate ? pool_error() : first_error(act_in)) return rc;
     {
       // predict / point-cloud bookkeeping on the host (the nominal state is already propagated)
       HostScope hs("predict");
@@ -1317,9 +1431,12 @@ class Batch {
           e.tracker_update_pointcloud(m.ids, m.xp_depth);
           if (m.type == 4 && !e.error) e.tracker_only_finish();
         }
-      });
+      }, [&](int i) { return act_in[i]; });
     }
-    if (int rc = first_error(act_in)) return rc;
+    if (isolate) {
+      if (int rc = pool_error()) return rc;
+      for (size_t i = 0; i < act_in.size(); ++i) proceed[i] = proceed[i] && !est[act_in[i]]->error;
+    } else if (int rc = first_error(act_in)) return rc;
     for (size_t i = 0; i < act_in.size(); ++i) {
       if (!proceed[i]) continue;
       const int b = act_in[i];
@@ -1331,9 +1448,10 @@ class Batch {
     if (int rc = integrate(full)) return rc;
     if (!lk_act.empty()) {
       if (int rc = est[0]->tc.match_tracker ? tracker_update_match(lk_act, lk_slots) : tracker_update_lk(lk_act, lk_slots)) return rc;
-      if (int rc = first_error(lk_act)) return rc;
+      if (int rc = settle(lk_act)) return rc;
+      prune(full);
       for (size_t i = 0; i < act_in.size(); ++i)
-        if (proceed[i] && msgs[i].type == 2) est[act_in[i]]->tracker_only_finish();
+        if (proceed[i] && msgs[i].type == 2 && !seq_failed(act_in[i])) est[act_in[i]]->tracker_only_finish();
     }
     if (full.empty()) return 0;
 
@@ -1342,6 +1460,12 @@ class Batch {
     {
       HostScope hs("process_tracks");
       pfor(full, [&](int b, int) { est[b]->update_step_pre(); });
+      if (isolate) {  // one sequence's sub-filter list over its share of the packed table
+        for (int b : full)
+          if ((int)est[b]->subfilter_list.size() > max_sub) fail_sequence(b, XIVO_ERR_STATE, "sub-filter list exceeds capacity");
+        if (int rc = settle(full)) return rc;
+        if (full.empty()) return 0;
+      }
       int nsub = 0;
       for (int b : full) {
         if ((int)est[b]->subfilter_list.size() > max_sub) return fail(XIVO_ERR_STATE, "sub-filter list exceeds capacity");
@@ -1406,14 +1530,20 @@ class Batch {
           const size_t fi = (size_t)b * lay.F + i;
           memcpy(fx.h + 3 * fi, f->x, 24);
           fxp.h[2 * fi] = f->xp()[0]; fxp.h[2 * fi + 1] = f->xp()[1];
-          if (f->ref->sind < 0 || f->sind < 0) { bad_slot = 1; return; }
+          if (f->ref->sind < 0 || f->sind < 0) {
+            if (isolate) fail_sequence(b, XIVO_ERR_STATE, "in-state feature without state slot");
+            else bad_slot = 1;
+            return;
+          }
           fref.h[fi] = f->ref->sind;
           fsind.h[fi] = f->sind;
         }
       });
-      if (int rc = first_error(full)) return rc;
+      if (int rc = settle(full)) return rc;
       if (bad_slot) return fail(XIVO_ERR_STATE, "in-state feature without state slot");
       if (int rc = stage_edits(full, opsJ, firstJ, nopsJ, &nops_total)) return rc;
+      prune(full);
+      if (isolate && full.empty()) return 0;
     }
     std::unique_ptr<HostScope> hs_issue(new HostScope("issue_jacobian"));
     // one copy: [nfeat | nops | first | fref | fsind | fxp | fx | groups | packed edit list]; the kernel applies the edits, then the features
@@ -1439,7 +1569,7 @@ class Batch {
         table_order[b] = e.instate_features;  // index space of mh / the device feature table
         e.update_step_after_gate(mh.h + (size_t)b * lay.F, use_1pt ? mh.h + (size_t)B * lay.F + (size_t)b * N : nullptr);
       });
-      if (int rc = first_error(full)) return rc;
+      if (int rc = settle(full)) return rc;
     }
     if (use_1pt) {  // Estimator::OnePointRANSAC's two device phases for the sequences whose gate asked for them (ransac.active)
       bool any = false;
@@ -1462,8 +1592,10 @@ class Batch {
         }
         nsel.h[b] = k;
       });
-      if (int rc = first_error(full)) return rc;
+      if (int rc = settle(full)) return rc;
       if (int rc = stage_edits(full, opsU, firstU, nopsU, &nops_total)) return rc;
+      prune(full);
+      if (isolate && full.empty()) return 0;
     }
     hs_issue.reset(new HostScope("issue_update"));
     XB_CUDA(up_blob(blobU, blobU_fixed + (size_t)nops_total * sizeof(EditOp), st));  // [nsel | nops | first | sel | packed post-gate edit list]
@@ -1492,13 +1624,14 @@ class Batch {
         if (notpd && !e.error) { e.error = XIVO_ERR_STATE; e.error_msg = "innovation covariance not positive definite"; }
       });
     }
-    return first_error(full);
+    return settle(full);
   }
 
   // Several messages per sequence in one call (same semantics as pushing them one by one): every
   // sequence runs ahead through its IMU messages until its heap releases a visual message; those are
   // then processed together, and the loop continues with the remaining messages.
-  // A sequence with no message (xivo_batch_feed) is not touched.
+  // A sequence with no message (xivo_batch_feed) is not touched, nor is a failed sequence of an isolating handle: the rest of its
+  // messages are dropped from the moment it fails.
   int ingest_many(std::vector<std::vector<Msg>>& in) {
     WorkPool::get().pin_driver();
     std::vector<int> all(B), fed, vis;
@@ -1507,9 +1640,17 @@ class Batch {
     std::vector<char> has(B, 0);
     for (int b = 0; b < B; ++b) {
       all[b] = b;
-      if (!in[b].empty()) fed.push_back(b);
+      if (!in[b].empty() && !seq_failed(b)) fed.push_back(b);
     }
     for (;;) {
+      if (isolate) {
+        size_t k = 0;
+        for (int b : fed) {
+          if (est[b]->error) has[b] = 0;
+          else fed[k++] = b;
+        }
+        fed.resize(k);
+      }
       {
         HostScope hs("ingest_imu");
         pfor(fed, [&](int b, int) {
@@ -1521,12 +1662,17 @@ class Batch {
             if (!est[b]->pop_ready(&m)) continue;
             if (m.type == 0) {
               est[b]->inertial_internal(m.ts, m.gyro, m.accel);
+              if (isolate && est[b]->error) return;
               if (est[b]->needs_state_now()) { has[b] = 2; return; }  // integrate on the device before going on
             } else { popped[b] = std::move(m); has[b] = 1; return; }
           }
         });
       }
-      if (int rc = first_error(all)) return rc;
+      if (isolate) {
+        if (int rc = pool_error()) return rc;
+        for (int b : fed)
+          if (est[b]->error) has[b] = 0;
+      } else if (int rc = first_error(all)) return rc;
       vis.clear();
       vmsgs.clear();
       std::vector<int> need_int;
@@ -1534,8 +1680,9 @@ class Batch {
       for (int b = 0; b < B; ++b) {
         if (has[b] == 1) { vis.push_back(b); vmsgs.push_back(std::move(popped[b])); }
         if (has[b] == 2) need_int.push_back(b);
-        more = more || pos[b] < in[b].size();
       }
+      for (int b : fed)
+        if (!seq_failed(b)) more = more || pos[b] < in[b].size();
       if (!need_int.empty())
         if (int rc = integrate(need_int)) return rc;
       if (vis.empty()) {
@@ -1546,13 +1693,13 @@ class Batch {
     }
   }
 
-  // Push one message per sequence, then execute whatever each heap releases (MaintainBuffer).
+  // Push one message per sequence, then execute whatever each heap releases (MaintainBuffer).  The message of a failed sequence of an
+  // isolating handle is dropped.
   int ingest(std::vector<Msg>& in) {
     WorkPool::get().pin_driver();
-    std::vector<int> all(B), vis;
+    std::vector<int> all = live_sequences(), vis;
     std::vector<Msg> popped(B), vmsgs;
     std::vector<char> has(B, 0);
-    for (int b = 0; b < B; ++b) all[b] = b;
     {
       HostScope hs("ingest_imu");
       pfor(all, [&](int b, int) {
@@ -1563,7 +1710,11 @@ class Batch {
         else { popped[b] = std::move(m); has[b] = 1; }
       });
     }
-    if (int rc = first_error(all)) return rc;
+    if (isolate) {
+      if (int rc = pool_error()) return rc;
+      for (int b : all)
+        if (est[b]->error) has[b] = 0;
+    } else if (int rc = first_error(all)) return rc;
     std::vector<int> need_int;
     for (int b = 0; b < B; ++b) {
       if (has[b] == 1) { vis.push_back(b); vmsgs.push_back(std::move(popped[b])); }
@@ -1604,6 +1755,12 @@ struct xivo_batch : Batch {
     set_error("sequence index %d out of range", seq); \
     return XIVO_ERR_ARG;                              \
   }
+// the state getters of a failed sequence of an isolating handle refuse with its message
+#define SEQ_LIVE                                                                                           \
+  if (B_.seq_failed(seq)) {                                                                                \
+    set_error("sequence %d has failed (%s); reset it to use it again", seq, B_.est[seq]->error_msg.c_str()); \
+    return XIVO_ERR_STATE;                                                                                 \
+  }
 
 extern "C" {
 
@@ -1640,6 +1797,8 @@ int xivo_batch_lanes(const xivo_batch* b) { return b ? 1 : 0; }
 int xivo_batch_inertial_meas(xivo_batch* b, const uint64_t* ts_ns, const double* gyro, const double* accel) {
   BATCH_BEGIN;
   XB_REQUIRE(ts_ns && gyro && accel, "inertial_meas: null argument");
+  if (int rc = B_.begin_call("inertial_meas")) return rc;
+  const int failed0 = B_.n_failed();
   std::vector<Msg> in(B_.B);
   for (int s = 0; s < B_.B; ++s) {
     in[s].ts = ts_ns[s];
@@ -1647,7 +1806,7 @@ int xivo_batch_inertial_meas(xivo_batch* b, const uint64_t* ts_ns, const double*
     memcpy(in[s].gyro, gyro + 3 * (size_t)s, 24);
     memcpy(in[s].accel, accel + 3 * (size_t)s, 24);
   }
-  return B_.ingest(in);
+  return B_.end_call(B_.ingest(in), failed0);
 }
 
 static int visual_meas_impl(xivo_batch* b, const uint64_t* ts_ns, const uint8_t* const* imgs, int rows, int cols, int channels,
@@ -1655,23 +1814,25 @@ static int visual_meas_impl(xivo_batch* b, const uint64_t* ts_ns, const uint8_t*
   BATCH_BEGIN;
   XB_REQUIRE(ts_ns && imgs && rows > 0 && cols > 0, "visual_meas: bad arguments");
   for (int s = 0; s < B_.B; ++s) XB_REQUIRE(imgs[s], "visual_meas: null image");
+  if (int rc = B_.begin_call("visual_meas")) return rc;
   if (int rc = B_.ensure_images(rows, cols, channels)) return rc;
+  const int failed0 = B_.n_failed();
   const size_t ib = (size_t)rows * cols * channels;
   std::vector<Msg> in(B_.B);
   std::vector<int> slot_of(B_.B);
   bool uploaded = false;
-  B_.take_slots(imgs, on_device, slot_of, &uploaded);
+  const std::vector<int> all = B_.live_sequences();
+  B_.take_slots(imgs, on_device, all, slot_of, &uploaded);
   for (int s = 0; s < B_.B; ++s) {
     in[s].ts = ts_ns[s];
     in[s].type = tracker_only ? 2 : 1;
     in[s].img_slot = slot_of[s];
   }
-  const std::vector<int> all = B_.every_sequence();
   if (!uploaded)
-    if (int rc = B_.upload_frames(imgs, all, slot_of, on_device, ib)) return rc;
+    if (int rc = B_.upload_frames(imgs, all, slot_of, on_device, ib)) return B_.end_call(rc, failed0);
   const int rc = B_.ingest(in);
   const int rc2 = B_.ingest_done(all, slot_of);
-  return rc ? rc : rc2;
+  return B_.end_call(rc ? rc : rc2, failed0);
 }
 
 int xivo_batch_visual_meas(xivo_batch* b, const uint64_t* ts_ns, const uint8_t* const* imgs, int rows, int cols, int channels,
@@ -1688,16 +1849,18 @@ int xivo_batch_visual_meas_png(xivo_batch* b, const uint64_t* ts_ns, const uint8
   XB_REQUIRE(ts_ns && png && png_bytes, "visual_meas_png: bad arguments");
   for (int s = 0; s < B_.B; ++s) XB_REQUIRE(png[s], "visual_meas_png: null data");
   if (channels != 1 && channels != 3) return B_.fail(XIVO_ERR_ARG, "visual_meas_png: channels must be 1 or 3, got " + std::to_string(channels));
+  if (int rc = B_.begin_call("visual_meas_png")) return rc;
   HostScope ht("visual_meas_png_total");
+  const int failed0 = B_.n_failed();
   std::vector<int> slot_of(B_.B);
-  if (int rc = B_.decode_png_frames(B_.every_sequence(), png, png_bytes, channels, slot_of)) return rc;
+  if (int rc = B_.decode_png_frames(B_.live_sequences(), png, png_bytes, channels, slot_of)) return rc;
   std::vector<Msg> in(B_.B);
   for (int s = 0; s < B_.B; ++s) {
     in[s].ts = ts_ns[s];
     in[s].type = tracker_only ? 2 : 1;
     in[s].img_slot = slot_of[s];
   }
-  return B_.ingest(in);
+  return B_.end_call(B_.ingest(in), failed0);
 }
 int xivo_batch_step(xivo_batch* b, int n_imu, const uint64_t* imu_ts, const double* gyro, const double* accel, const uint64_t* frame_ts,
                     const uint8_t* const* imgs, int rows, int cols, int channels, int on_device) {
@@ -1705,13 +1868,16 @@ int xivo_batch_step(xivo_batch* b, int n_imu, const uint64_t* imu_ts, const doub
   XB_REQUIRE(n_imu >= 0 && frame_ts && imgs && (n_imu == 0 || (imu_ts && gyro && accel)), "batch_step: bad arguments");
   const int nb = B_.B;  // the IMU arrays are (n_imu, nb[, 3])
   for (int s = 0; s < nb; ++s) XB_REQUIRE(imgs[s], "batch_step: null image");
+  if (int rc = B_.begin_call("batch_step")) return rc;
   HostScope hst("ingest_many_total");
   if (int rc = B_.ensure_images(rows, cols, channels)) return rc;
+  const int failed0 = B_.n_failed();
   const size_t ib = (size_t)rows * cols * channels;
   std::vector<std::vector<Msg>> in(nb);
   std::vector<int> slot_of(nb);
   bool uploaded = false;
-  B_.take_slots(imgs, on_device != 0, slot_of, &uploaded);
+  const std::vector<int> all = B_.live_sequences();
+  B_.take_slots(imgs, on_device != 0, all, slot_of, &uploaded);
   {
     HostScope hm("marshal");
     for (int s = 0; s < nb; ++s) {
@@ -1730,12 +1896,11 @@ int xivo_batch_step(xivo_batch* b, int n_imu, const uint64_t* imu_ts, const doub
       v.img_slot = slot_of[s];
     }
   }
-  const std::vector<int> all = B_.every_sequence();
   if (!uploaded)
-    if (int rc = B_.upload_frames(imgs, all, slot_of, on_device != 0, ib)) return rc;
+    if (int rc = B_.upload_frames(imgs, all, slot_of, on_device != 0, ib)) return B_.end_call(rc, failed0);
   const int rc = B_.ingest_many(in);
   const int rc2 = B_.ingest_done(all, slot_of);
-  return rc ? rc : rc2;
+  return B_.end_call(rc ? rc : rc2, failed0);
 }
 
 // xivo_batch_feed[_png]: what is refused is refused here, before a ring slot is taken or a message pushed.
@@ -1780,11 +1945,12 @@ int xivo_batch_feed(xivo_batch* b, const int* n_imu, const uint64_t* imu_ts, con
                     const uint8_t* const* imgs, int rows, int cols, int channels, int on_device, int tracker_only) {
   BATCH_BEGIN;
   HostScope hst("feed_total");
-  std::vector<int> present;  // the sequences that get a frame
+  std::vector<int> present;  // the sequences that get a frame (a failed sequence of an isolating handle gets none)
   if (imgs)
     for (int s = 0; s < B_.B; ++s)
-      if (imgs[s]) present.push_back(s);
+      if (imgs[s] && !B_.seq_failed(s)) present.push_back(s);
   if (int rc = feed_check(B_, "feed", n_imu, imu_ts, gyro, accel, frame_ts, !present.empty())) return rc;
+  const int failed0 = B_.n_failed();
   std::vector<int> slot_of(B_.B, -1);
   const size_t ib = (size_t)rows * cols * channels;
   if (!present.empty()) {
@@ -1796,13 +1962,13 @@ int xivo_batch_feed(xivo_batch* b, const int* n_imu, const uint64_t* imu_ts, con
     if (int rc = B_.ensure_images(rows, cols, channels)) return rc;
     B_.drop_prefetches();
     B_.fresh_slots(present, slot_of);
-    if (int rc = B_.upload_frames(imgs, present, slot_of, on_device != 0, ib)) return rc;
+    if (int rc = B_.upload_frames(imgs, present, slot_of, on_device != 0, ib)) return B_.end_call(rc, failed0);
   }
   std::vector<std::vector<Msg>> in(B_.B);
   feed_messages(B_, n_imu, imu_ts, gyro, accel, frame_ts, present, slot_of, tracker_only, in);
   const int rc = B_.ingest_many(in);
   const int rc2 = present.empty() ? 0 : B_.ingest_done(present, slot_of);
-  return rc ? rc : rc2;
+  return B_.end_call(rc ? rc : rc2, failed0);
 }
 
 int xivo_batch_feed_png(xivo_batch* b, const int* n_imu, const uint64_t* imu_ts, const double* gyro, const double* accel, const uint64_t* frame_ts,
@@ -1812,8 +1978,9 @@ int xivo_batch_feed_png(xivo_batch* b, const int* n_imu, const uint64_t* imu_ts,
   std::vector<int> present;
   if (png)
     for (int s = 0; s < B_.B; ++s)
-      if (png[s]) present.push_back(s);
+      if (png[s] && !B_.seq_failed(s)) present.push_back(s);
   if (int rc = feed_check(B_, "feed_png", n_imu, imu_ts, gyro, accel, frame_ts, !present.empty())) return rc;
+  const int failed0 = B_.n_failed();
   std::vector<int> slot_of(B_.B, -1);
   if (!present.empty()) {
     if (!png_bytes) return B_.fail(XIVO_ERR_ARG, "feed_png: null png_bytes");
@@ -1822,7 +1989,7 @@ int xivo_batch_feed_png(xivo_batch* b, const int* n_imu, const uint64_t* imu_ts,
   }
   std::vector<std::vector<Msg>> in(B_.B);
   feed_messages(B_, n_imu, imu_ts, gyro, accel, frame_ts, present, slot_of, tracker_only, in);
-  return B_.ingest_many(in);
+  return B_.end_call(B_.ingest_many(in), failed0);
 }
 
 int xivo_batch_prefetch_frames(xivo_batch* b, const uint8_t* const* imgs, int rows, int cols, int channels) {
@@ -1855,14 +2022,17 @@ int xivo_batch_visual_meas_pointcloud(xivo_batch* b, const uint64_t* ts_ns, cons
                                       const double* const* xp_depth, int tracker_only) {
   BATCH_BEGIN;
   XB_REQUIRE(ts_ns && n_pts && ids && xp_depth, "visual_meas_pointcloud: null argument");
+  if (int rc = B_.begin_call("visual_meas_pointcloud")) return rc;
+  const int failed0 = B_.n_failed();
   std::vector<Msg> in(B_.B);
   for (int s = 0; s < B_.B; ++s) {
+    if (B_.seq_failed(s)) continue;
     in[s].ts = ts_ns[s];
     in[s].type = tracker_only ? 4 : 3;
     in[s].ids.assign(ids[s], ids[s] + n_pts[s]);
     in[s].xp_depth.assign(xp_depth[s], xp_depth[s] + 3 * (size_t)n_pts[s]);
   }
-  return B_.ingest(in);
+  return B_.end_call(B_.ingest(in), failed0);
 }
 
 static void put34(const SE3h& g, double* out) {
@@ -1872,18 +2042,18 @@ static void put34(const SE3h& g, double* out) {
   }
 }
 int xivo_get_gsb(xivo_batch* b, int seq, double* out) {
-  BATCH_BEGIN; SEQ_CHECK;
+  BATCH_BEGIN; SEQ_CHECK; SEQ_LIVE;
   put34(B_.est[seq]->gsb(), out);
   return 0;
 }
-int xivo_get_gbc(xivo_batch* b, int seq, double* out) { BATCH_BEGIN; SEQ_CHECK; put34(B_.est[seq]->gbc(), out); return 0; }
+int xivo_get_gbc(xivo_batch* b, int seq, double* out) { BATCH_BEGIN; SEQ_CHECK; SEQ_LIVE; put34(B_.est[seq]->gbc(), out); return 0; }
 int xivo_get_gsc(xivo_batch* b, int seq, double* out) {
-  BATCH_BEGIN; SEQ_CHECK;
+  BATCH_BEGIN; SEQ_CHECK; SEQ_LIVE;
   put34(se3_mul(B_.est[seq]->gsb(), B_.est[seq]->gbc()), out);
   return 0;
 }
 int xivo_get_motion(xivo_batch* b, int seq, double* Vsb, double* bg, double* ba, double* Rsg) {
-  BATCH_BEGIN; SEQ_CHECK;
+  BATCH_BEGIN; SEQ_CHECK; SEQ_LIVE;
   const MotionX& X = B_.est[seq]->X;
   if (Vsb) memcpy(Vsb, X.Vsb.v, 24);
   if (bg) memcpy(bg, X.bg.v, 24);
@@ -1892,21 +2062,23 @@ int xivo_get_motion(xivo_batch* b, int seq, double* Vsb, double* bg, double* ba,
   return 0;
 }
 int xivo_get_P(xivo_batch* b, int seq, double* out) {
-  BATCH_BEGIN; SEQ_CHECK;
+  BATCH_BEGIN; SEQ_CHECK; SEQ_LIVE;
   XB_REQUIRE(out, "get_P: null output");
   if (int rc = B_.flush({seq})) return rc;
+  SEQ_LIVE;  // its share of the edit list may have overflowed
   XB_CUDA(cudaMemcpy(out, B_.dP.p + (size_t)seq * B_.N * B_.N, sizeof(double) * B_.N * B_.N, cudaMemcpyDeviceToHost));
   return 0;
 }
 int xivo_get_Pstate(xivo_batch* b, int seq, double* out81) {
-  BATCH_BEGIN; SEQ_CHECK;
+  BATCH_BEGIN; SEQ_CHECK; SEQ_LIVE;
   if (int rc = B_.flush({seq})) return rc;
+  SEQ_LIVE;  // its share of the edit list may have overflowed
   for (int i = 0; i < 9; ++i)
     XB_CUDA(cudaMemcpy(out81 + 9 * i, B_.dP.p + (size_t)seq * B_.N * B_.N + (size_t)i * B_.N, sizeof(double) * 9, cudaMemcpyDeviceToHost));
   return 0;
 }
 int xivo_get_counters(xivo_batch* b, int seq, int* out) {
-  BATCH_BEGIN; SEQ_CHECK;
+  BATCH_BEGIN; SEQ_CHECK; SEQ_LIVE;
   Estimator& e = *B_.est[seq];
   int ng = 0;
   for (auto& kv : e.graph.groups) ng += kv.second->instate();
@@ -1924,9 +2096,9 @@ int xivo_get_counters(xivo_batch* b, int seq, int* out) {
   out[11] = e.error;
   return 0;
 }
-int xivo_get_time_ns(xivo_batch* b, int seq, uint64_t* ts) { BATCH_BEGIN; SEQ_CHECK; *ts = B_.est[seq]->curr_time; return 0; }
+int xivo_get_time_ns(xivo_batch* b, int seq, uint64_t* ts) { BATCH_BEGIN; SEQ_CHECK; SEQ_LIVE; *ts = B_.est[seq]->curr_time; return 0; }
 int xivo_get_tracked_features(xivo_batch* b, int seq, int* ids, double* xy, int* status, int max_n, int* n) {
-  BATCH_BEGIN; SEQ_CHECK;
+  BATCH_BEGIN; SEQ_CHECK; SEQ_LIVE;
   int k = 0;
   for (Feature* f : B_.est[seq]->tracks) {
     if (k < max_n) {
@@ -1940,7 +2112,7 @@ int xivo_get_tracked_features(xivo_batch* b, int seq, int* ids, double* xy, int*
   return 0;
 }
 int xivo_get_tracked_descriptors(xivo_batch* b, int seq, uint8_t* desc, uint8_t* has, int max_n, int* n) {
-  BATCH_BEGIN; SEQ_CHECK;
+  BATCH_BEGIN; SEQ_CHECK; SEQ_LIVE;
   XB_REQUIRE(n, "get_tracked_descriptors: null count");
   int k = 0;
   for (Feature* f : B_.est[seq]->tracks) {
@@ -1954,7 +2126,7 @@ int xivo_get_tracked_descriptors(xivo_batch* b, int seq, uint8_t* desc, uint8_t*
   return 0;
 }
 int xivo_get_instate_features(xivo_batch* b, int seq, int* ids, int* sinds, int* refs, double* Xs3, double* x3, int max_n, int* n) {
-  BATCH_BEGIN; SEQ_CHECK;
+  BATCH_BEGIN; SEQ_CHECK; SEQ_LIVE;
   Estimator& e = *B_.est[seq];
   int k = 0;
   for (Feature* f : e.instate_features) {
@@ -1976,7 +2148,7 @@ int xivo_get_instate_features(xivo_batch* b, int seq, int* ids, int* sinds, int*
   return 0;
 }
 int xivo_get_instate_groups(xivo_batch* b, int seq, int* ids, int* sinds, double* gsb12, int max_n, int* n) {
-  BATCH_BEGIN; SEQ_CHECK;
+  BATCH_BEGIN; SEQ_CHECK; SEQ_LIVE;
   int k = 0;
   for (auto& kv : B_.est[seq]->graph.groups) {
     Group* g = kv.second;
@@ -1995,12 +2167,13 @@ int xivo_get_instate_groups(xivo_batch* b, int seq, int* ids, int* sinds, double
 static int fetch_P(Batch& B_, int seq, std::vector<double>* P) {
   P->resize((size_t)B_.N * B_.N);
   if (int rc = B_.flush({seq})) return rc;
+  SEQ_LIVE;  // its share of the edit list may have overflowed
   XB_CUDA(cudaMemcpy(P->data(), B_.dP.p + (size_t)seq * B_.N * B_.N, sizeof(double) * B_.N * B_.N, cudaMemcpyDeviceToHost));
   return 0;
 }
 int xivo_get_instate_feature_table(xivo_batch* b, int seq, int n_output, int* ids, int* sinds, int* ref_group_ids, double* Xs3, double* Xc3,
                                    double* xc3, double* pred2, double* meas2, double* cov6, int max_n, int* n) {
-  BATCH_BEGIN; SEQ_CHECK;
+  BATCH_BEGIN; SEQ_CHECK; SEQ_LIVE;
   XB_REQUIRE(n, "get_instate_feature_table: null count");
   std::vector<double> P;
   if (int rc = fetch_P(B_, seq, &P)) return rc;
@@ -2021,7 +2194,7 @@ int xivo_get_instate_feature_table(xivo_batch* b, int seq, int n_output, int* id
   return 0;
 }
 int xivo_get_instate_group_table(xivo_batch* b, int seq, int* ids, int* sinds, double* pose7, double* cov36, int max_n, int* n) {
-  BATCH_BEGIN; SEQ_CHECK;
+  BATCH_BEGIN; SEQ_CHECK; SEQ_LIVE;
   XB_REQUIRE(n, "get_instate_group_table: null count");
   std::vector<double> P;
   if (int rc = fetch_P(B_, seq, &P)) return rc;
@@ -2036,7 +2209,7 @@ int xivo_get_instate_group_table(xivo_batch* b, int seq, int* ids, int* sinds, d
   return 0;
 }
 int xivo_get_calibration(xivo_batch* b, int seq, double* Ca9, double* Cg9, double* td, double* intrinsics9, int* distortion_type) {
-  BATCH_BEGIN; SEQ_CHECK;
+  BATCH_BEGIN; SEQ_CHECK; SEQ_LIVE;
   const Estimator& e = *B_.est[seq];
   if (Ca9) memcpy(Ca9, e.c.Ca.m, 72);
   if (Cg9) memcpy(Cg9, e.c.Cg.m, 72);
@@ -2050,7 +2223,7 @@ int xivo_get_calibration(xivo_batch* b, int seq, double* Ca9, double* Cg9, doubl
   return 0;
 }
 int xivo_get_just_dropped(xivo_batch* b, int seq, int* ids, int max_n, int* n) {
-  BATCH_BEGIN; SEQ_CHECK;
+  BATCH_BEGIN; SEQ_CHECK; SEQ_LIVE;
   XB_REQUIRE(n, "get_just_dropped: null count");
   const std::vector<int>& v = B_.est[seq]->just_dropped_ids;
   for (size_t i = 0; i < v.size() && (int)i < max_n; ++i)
@@ -2059,7 +2232,7 @@ int xivo_get_just_dropped(xivo_batch* b, int seq, int* ids, int max_n, int* n) {
   return 0;
 }
 int xivo_get_tracker_counters(xivo_batch* b, int seq, int out[4]) {
-  BATCH_BEGIN; SEQ_CHECK;
+  BATCH_BEGIN; SEQ_CHECK; SEQ_LIVE;
   const Estimator& e = *B_.est[seq];
   out[0] = e.num_outliers_rejected;  // Tracker::num_rejected_outliers()
   out[1] = e.num_failed_to_track;
@@ -2068,7 +2241,7 @@ int xivo_get_tracker_counters(xivo_batch* b, int seq, int out[4]) {
   return 0;
 }
 int xivo_scale_init_velocity(xivo_batch* b, int seq, double scale) {  // Estimator::ScaleInitVelocity: X_.Vsb /= scale
-  BATCH_BEGIN; SEQ_CHECK;
+  BATCH_BEGIN; SEQ_CHECK; SEQ_LIVE;
   Estimator& e = *B_.est[seq];
   for (int k = 0; k < 3; ++k) e.X.Vsb.v[k] /= scale;
   return 0;
@@ -2091,6 +2264,31 @@ int xivo_batch_reset_sequence(xivo_batch* b, int seq, const char* cfg_json) {
     return XIVO_ERR_ARG;
   }
   return B_.reset_sequence(seq, &cfg);
+}
+int xivo_batch_isolate_failures(xivo_batch* b, int on) {
+  if (!b) {
+    set_error("null batch");
+    return XIVO_ERR_ARG;
+  }
+  return b->set_isolation(on != 0);
+}
+int xivo_batch_sequence_status(const xivo_batch* b, int seq, int* code, char* msg, int msg_cap) {
+  if (!b || !code) {
+    set_error("sequence_status: null argument");
+    return XIVO_ERR_ARG;
+  }
+  if (seq < 0 || seq >= b->B) {
+    set_error("sequence index %d out of range", seq);
+    return XIVO_ERR_ARG;
+  }
+  const Estimator& e = *b->est[seq];
+  *code = e.error;
+  if (msg && msg_cap > 0) {
+    const size_t n = std::min(e.error ? e.error_msg.size() : 0, (size_t)msg_cap - 1);
+    memcpy(msg, e.error_msg.data(), n);
+    msg[n] = 0;
+  }
+  return XIVO_OK;
 }
 const char* xivo_batch_error(xivo_batch* b, int seq) {
   if (!b || seq < 0 || seq >= b->B) return "";

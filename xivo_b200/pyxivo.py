@@ -52,7 +52,12 @@ def _cfg_text(cfg, overrides=None) -> str:
 
 
 class Batch:
-    def __init__(self, cfg, n_seq=1, max_groups=15, max_features=30, tracker_only=False, device=0, ctx=None, overrides=None):
+    """n_seq sequences in one handle.  isolate_failures=True confines a sequence's failure to that sequence
+    (xivo_batch_isolate_failures): the message methods then do not raise when sequences fail during a call (failed() lists them, and
+    their state getters raise until reset_sequence brings them back); a handle-wide failure still raises."""
+
+    def __init__(self, cfg, n_seq=1, max_groups=15, max_features=30, tracker_only=False, device=0, ctx=None, overrides=None,
+                 isolate_failures=False):
         text = _cfg_text(cfg, overrides)
         self.cfg = json.loads(text)
         self._own_ctx = ctx is None
@@ -68,6 +73,9 @@ class Batch:
         self._keep = None
         cam = self.cfg.get("camera_cfg") if isinstance(self.cfg.get("camera_cfg"), dict) else None
         self._cam_shape = (int(cam["rows"]), int(cam["cols"])) if cam and "rows" in cam and "cols" in cam else None
+        self.isolate_failures = False
+        if isolate_failures:
+            self.set_isolate_failures(True)
 
     def close(self):
         if self._h:
@@ -83,12 +91,34 @@ class Batch:
         except Exception:
             pass
 
+    # ---- failure isolation ----------------------------------------------------------------
+    def set_isolate_failures(self, on=True):
+        """Turn failure isolation on or off (xivo_batch_isolate_failures); turning it off is refused while a sequence is failed."""
+        _check(capi.lib().xivo_batch_isolate_failures(self._h, int(bool(on))), "xivo_batch_isolate_failures")
+        self.isolate_failures = bool(on)
+
+    def status(self, seq):
+        """(code, message) of sequence `seq`: (0, "") while it runs, else its error code and message."""
+        code, msg = C.c_int(), C.create_string_buffer(1024)
+        _check(capi.lib().xivo_batch_sequence_status(self._h, int(seq), C.byref(code), msg, len(msg)), "xivo_batch_sequence_status")
+        return code.value, msg.value.decode(errors="replace")
+
+    def failed(self):
+        """{seq: (code, message)} of every failed sequence."""
+        return {s: st for s in range(self.n) for st in [self.status(s)] if st[0]}
+
+    def _msg(self, rc, what):
+        """A message call's result: XIVO_SEQ_FAILED is not an error on an isolating handle."""
+        if rc == capi.XIVO_SEQ_FAILED and self.isolate_failures:
+            return
+        _check(rc, what)
+
     # ---- ingest -------------------------------------------------------------------------
     def inertial_meas(self, ts_ns, gyro, accel):
         ts = np.ascontiguousarray(np.broadcast_to(np.asarray(ts_ns, dtype=np.uint64), (self.n,)))
         g = np.ascontiguousarray(np.broadcast_to(np.asarray(gyro, dtype=np.float64), (self.n, 3)))
         a = np.ascontiguousarray(np.broadcast_to(np.asarray(accel, dtype=np.float64), (self.n, 3)))
-        _check(capi.lib().xivo_batch_inertial_meas(self._h, _p(ts), _p(g), _p(a)), "xivo_batch_inertial_meas")
+        self._msg(capi.lib().xivo_batch_inertial_meas(self._h, _p(ts), _p(g), _p(a)), "xivo_batch_inertial_meas")
 
     def _check_images(self, imgs, count=None):
         """One image per sequence (or `count` images), all of the same shape (rows x cols [x 1 | 3]), uint8, C-contiguous: the C side reads
@@ -117,7 +147,7 @@ class Batch:
         ts = np.ascontiguousarray(np.broadcast_to(np.asarray(ts_ns, dtype=np.uint64), (self.n,)))
         ptrs = (C.c_void_p * self.n)(*[i.ctypes.data for i in imgs])
         self._keep = imgs
-        _check(capi.lib().xivo_batch_visual_meas(self._h, _p(ts), ptrs, rows, cols, ch, int(bool(tracker_only))), "xivo_batch_visual_meas")
+        self._msg(capi.lib().xivo_batch_visual_meas(self._h, _p(ts), ptrs, rows, cols, ch, int(bool(tracker_only))), "xivo_batch_visual_meas")
 
     def visual_meas_png(self, ts_ns, blobs, channels=3, tracker_only=False):
         """visual_meas with the frames given as PNG file bytes (one per sequence, or one shared by all), decoded on the device straight
@@ -131,7 +161,7 @@ class Batch:
         ts = np.ascontiguousarray(np.broadcast_to(np.asarray(ts_ns, dtype=np.uint64), (self.n,)))
         src = (C.c_char_p * self.n)(*blobs)
         sizes = (C.c_size_t * self.n)(*[len(x) for x in blobs])
-        _check(capi.lib().xivo_batch_visual_meas_png(self._h, _p(ts), src, sizes, int(channels), int(bool(tracker_only))), "xivo_batch_visual_meas_png")
+        self._msg(capi.lib().xivo_batch_visual_meas_png(self._h, _p(ts), src, sizes, int(channels), int(bool(tracker_only))), "xivo_batch_visual_meas_png")
 
     def prefetch_frames(self, imgs):
         """Start uploading the frames of the NEXT visual_meas / step call (same arrays) while the current one is computed."""
@@ -152,7 +182,7 @@ class Batch:
         fts = np.ascontiguousarray(np.broadcast_to(np.asarray(frame_ts, dtype=np.uint64), (self.n,)))
         ptrs = (C.c_void_p * self.n)(*[i.ctypes.data for i in imgs])
         self._keep = imgs
-        _check(capi.lib().xivo_batch_step(self._h, n_imu, _p(its), _p(g), _p(a), _p(fts), ptrs, rows, cols, ch, 0), "xivo_batch_step")
+        self._msg(capi.lib().xivo_batch_step(self._h, n_imu, _p(its), _p(g), _p(a), _p(fts), ptrs, rows, cols, ch, 0), "xivo_batch_step")
 
     def _feed_imu(self, imu):
         """-> n_imu (n,), imu_ts, gyro, accel: the per-sequence samples concatenated in sequence order."""
@@ -215,7 +245,7 @@ class Batch:
                 for (s, _), i in zip(present, imgs):
                     ptrs[s] = i.ctypes.data
                 self._keep = imgs
-        _check(capi.lib().xivo_batch_feed(self._h, _p(n_imu), _p(its), _p(g), _p(a), _p(fts), ptrs, rows, cols, ch, on_device, int(bool(tracker_only))),
+        self._msg(capi.lib().xivo_batch_feed(self._h, _p(n_imu), _p(its), _p(g), _p(a), _p(fts), ptrs, rows, cols, ch, on_device, int(bool(tracker_only))),
                "xivo_batch_feed")
 
     def feed_png(self, imu, frames, channels=3, tracker_only=False):
@@ -229,7 +259,7 @@ class Batch:
         for (s, _), b in zip(present, blobs):
             src[s] = b
             sizes[s] = len(b)
-        _check(capi.lib().xivo_batch_feed_png(self._h, _p(n_imu), _p(its), _p(g), _p(a), _p(fts), src, sizes, int(channels), int(bool(tracker_only))),
+        self._msg(capi.lib().xivo_batch_feed_png(self._h, _p(n_imu), _p(its), _p(g), _p(a), _p(fts), src, sizes, int(channels), int(bool(tracker_only))),
                "xivo_batch_feed_png")
 
     def visual_meas_pointcloud(self, ts_ns, ids, xp_depth, tracker_only=False):
@@ -247,7 +277,7 @@ class Batch:
         ts = np.ascontiguousarray(np.broadcast_to(np.asarray(ts_ns, dtype=np.uint64), (self.n,)))
         pi = (C.c_void_p * self.n)(*[i.ctypes.data for i in ids])
         px = (C.c_void_p * self.n)(*[x.ctypes.data for x in xpd])
-        _check(capi.lib().xivo_batch_visual_meas_pointcloud(self._h, _p(ts), _p(npts), pi, px, int(bool(tracker_only))),
+        self._msg(capi.lib().xivo_batch_visual_meas_pointcloud(self._h, _p(ts), _p(npts), pi, px, int(bool(tracker_only))),
                "xivo_batch_visual_meas_pointcloud")
 
     def init_with_sim_depths(self):
